@@ -68,6 +68,12 @@
 #ifndef LHW_BLOCK_SYNC
 #define LHW_BLOCK_SYNC(on) ((void)0)
 #endif
+// Newton-step census (tools/newton_census.py): only the census build of the CPU emulation (tools/newton_census.cpp) defines
+// this hook; the product compiles none of it.
+// Events: 0 = solve starts, 1 = line-search evaluation number n (0 = at alpha 0), 2 = solve done (w.iters_total has the steps)
+#ifndef LHW_NEWTON_HOOK
+#define LHW_NEWTON_HOOK(event, w, n) ((void)0)
+#endif
 #if defined(__CUDA_ARCH__) && !defined(LHW_CPU_EMU)
 #define LHW_ASSUME_SHARED(p) __builtin_assume(__isShared(p))
 #else
@@ -710,7 +716,8 @@ template <class real> LHW_DEV real floss_force(real D, real lim, real fl, real x
 
 // ================================================================= one physics substep (mujoco.mj_step)
 template <class real, int NJ, int TK>
-LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, const bool last, const int block_sync = 0) {
+LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, const bool last, const int block_sync = 0,
+                       const bool chained = false) {
   constexpr int NL = 1 + 2 * NJ, NV = 6 + 2 * NJ, NU = 2 * NJ, NA = 6 + NJ;
   constexpr int CPF = Cfg<NJ, TK>::CPF, NCON = 2 * CPF, NEDGE = 4 * NCON, NPTS = Cfg<NJ, TK>::NPTS;
   constexpr bool PERENV = Cfg<NJ, TK>::PERENV, FLOSS = Cfg<NJ, TK>::FLOSS;
@@ -1241,7 +1248,10 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
       }
       if (l >= 6) q += w.ctrl[l - 6];
       w.qfs[l] = q;
-      w.qacc[l] = w.qacc_warm[l];
+      // warm start: the last solution, extrapolated linearly from the one before it (in vec since P12) once the control step
+      // has had a substep; a_k + (a_k - a_{k-1}) starts the solve inside the final active set more often, so fewer substeps
+      // take a second Newton step -- and a lock-step block pays the largest count among its warps (DESIGN.md §4.1)
+      w.qacc[l] = chained ? 2 * w.qacc_warm[l] - w.vec[l] : w.qacc_warm[l];
     } else if (l < NV + NU) {
       const int u = l - NV, d = 6 + u;
       const real q = w.qpos[7 + u];
@@ -1286,6 +1296,7 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
   // ---------------- P10 primal Newton on  1/2 (a-a_s)' M (a-a_s) + sum_r 1/2 D_r min(0, J_r a - aref_r)^2
   // residuals (Ma, ejar, ljar) are carried incrementally: x += alpha * (direction image)
   bool converged = false;
+  LHW_NEWTON_HOOK(0, w, 0);
   for (int iter = 0; iter <= m.max_iter && !converged; iter++) {
     // (a) per contact: force in the contact frame and the 3x3 weight  W = sum_active D w w'  (lane = contact);
     // active set = sign of the carried residuals (inactive slots carry jar = 1)
@@ -1456,6 +1467,7 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
     const real LS_TOL = sizeof(real) == 8 ? (real)2e-14 : (real)1e-5;
     real alpha = 1, lo = 0, hi = -1, d_at0 = 0;
     for (int ls = 0; ls < 40; ls++) {
+      LHW_NEWTON_HOOK(1, w, ls);
       const real al = ls == 0 ? (real)0 : alpha;
       const real cd = warp_sum<real>([&](int l) {
         real acc = 0;
@@ -1479,7 +1491,9 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
         if (!(d < 0)) { alpha = 0; break; }  // not a descent direction: at the roundoff floor
         continue;                            // first trial: the full Newton step alpha = 1
       }
-      if (m_abs(d) <= LS_TOL * m_abs(d_at0)) break;
+      // done when phi' is zero relative to phi'(0), or to the size of the terms that cancel in it (the roundoff floor: a warm
+      // start close to the solution has a tiny phi'(0), and trials below that floor only chase rounding)
+      if (m_abs(d) <= LS_TOL * m_max(m_abs(d_at0), al * sMs + m_abs(sg) + m_abs(cd))) break;
       const real cdd = warp_sum<real>([&](int l) {
         real acc = 0;
         LHW_STRIDED(ed, l, NEDGE)
@@ -1515,6 +1529,7 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
     LHW_SYNC();
     if (alpha == 0) converged = true;
   }
+  LHW_NEWTON_HOOK(2, w, 0);
 
   // ---------------- P11 what mjData keeps after mj_step (evaluated at the pre-integration state)
   LHW_LANES(l) {
@@ -1626,6 +1641,7 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
     if (l < NV) {
       const real a = w.vec[l];
       if (!(m_abs(a) < (real)1e10)) w.status |= 1;
+      w.vec[l] = w.qacc_warm[l];   // a_{k-1} for the next substep's warm start (vec is free until P11)
       w.qacc_warm[l] = w.qacc[l];
       w.qvel[l] += m.h * a;
     }
@@ -2080,7 +2096,7 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
       if (l < NU) w.ctrl[l] = w.kp_step[l] * (w.target[l] - w.act_len[l]) + w.kd_step[l] * ((real)0 - w.act_vel[l]);
     }
     LHW_SYNC();
-    if (alive) substep<real, NJ, TK>(w, m, sidx == m.frame_skip - 1, block_sync);
+    if (alive) substep<real, NJ, TK>(w, m, sidx == m.frame_skip - 1, block_sync, sidx > 0);
     else LHW_BLOCK_SYNC(block_sync & 2);
     LHW_BLOCK_SYNC((block_sync & 1) && ((sidx + 1) % ((block_sync >> 4) + 1) == 0));   // every (block_sync>>4)+1 substeps
   }

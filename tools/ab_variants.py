@@ -24,6 +24,9 @@ BUILDS = {
     "base": [],
     # round 2, second batch (profiles/r02_ab_variants.md): "-DLHW_X_REGCAP=576 | 640 | 896" = 112 / 96 / 72 registers per thread of the
     # fp64 lock-step kernel (18 / 20 / 28 warps per SM) — measured, not adopted
+    # warm starts of the Newton solve, screened with tools/newton_census.py (DESIGN.md §4.1): the extrapolated warm start won on
+    # every workload and regime and is now the kernel; the active-set warm start (first Hessian from the previous solve's final
+    # active set), alone or with it, raised the block maximum everywhere and was deleted before any GPU timing
 }
 # (build, env knobs) timed on (model, precision, n_envs); runs with knobs only time the headline workload
 RUNS = [
