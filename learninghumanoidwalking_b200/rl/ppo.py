@@ -24,7 +24,9 @@ from torch.nn import functional as F
 
 from .. import _lib
 from .optim import FusedClipAdam
+from . import snapshot
 from .policies import FF_V, Gaussian_FF_Actor
+from .snapshot import SnapshotError, plain_args
 from .storage import BatchData
 from .workers import DeviceRolloutWorker
 
@@ -75,6 +77,10 @@ class PPO:
         self.steps_per_env = getattr(args, "steps_per_env", None) or self.max_traj_len
         self.total_steps, self.iteration_count = 0, 0
         self.save_path = Path(getattr(args, "logdir", "/tmp/lhw_b200_logs"))
+        # opt-in (`train --snapshot`): the whole training state at every checkpoint point, for `run_experiment.py resume`
+        self.write_snapshots = bool(getattr(args, "snapshot", False))
+        self._run_args = plain_args(args)
+        self._elapsed0 = 0.0                    # training time of the run before a restore()
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.rank = dist.get_rank() if self.world > 1 else 0
 
@@ -142,6 +148,85 @@ class PPO:
             self.old_policy.load_state_dict(self.policy.state_dict())
             self.old_policy.obs_mean.copy_(self.policy.obs_mean)
             self.old_policy.obs_std.copy_(self.policy.obs_std)
+
+    # ------------------------------------------------------------------ snapshots (rl/snapshot.py): resume a run bit for bit
+    def _inner_env(self):
+        """The batched env itself, not a SymmetricEnv wrapper around it (attribute writes must reach the env)."""
+        return self.env.__dict__.get("env", self.env)
+
+    def _fused_optimizers(self):
+        a_opt, c_opt = self.actor_optimizer, self.critic_optimizer
+        if not (isinstance(a_opt, FusedClipAdam) and isinstance(c_opt, FusedClipAdam)):
+            raise SnapshotError("snapshots cover the optimisers of make_optimizers() (FusedClipAdam over the flat buffer) only")
+        return a_opt, c_opt
+
+    def snapshot_learner(self, itr: int, elapsed: float) -> dict:
+        """The learner's part of the snapshot at the end of iteration `itr`: identical on every rank, written by rank 0."""
+        a_opt, c_opt = self._fused_optimizers()
+        if self._comm is not None:      # the fused exchange keeps one Adam step number for both networks in device memory
+            dev = [self._comm.status()[0]] * 2
+        else:
+            dev = [int(a_opt.step_dev.item()), int(c_opt.step_dev.item())]
+        cpu = lambda t: t.detach().cpu().clone()
+        return dict(format=snapshot.FORMAT, itr=int(itr), world=self.world, args=self._run_args,
+                    flat_param=cpu(self._flat_param), exp_avg=cpu(self._flat_m), exp_avg_sq=cpu(self._flat_v),
+                    step_count=[a_opt.step_count, c_opt.step_count], adam_step_dev=dev,
+                    obs_norm={f"{net}.{name}": cpu(getattr(getattr(self, net), name))
+                              for net in ("policy", "critic") for name in ("obs_mean", "obs_std")},
+                    best_eval=float(self._best_eval), total_steps=int(self.total_steps), elapsed=float(elapsed))
+
+    def snapshot_shard(self, itr: int) -> dict:
+        """This rank's part of the snapshot: its environments' records and its sampler's state."""
+        env = self._inner_env()
+        return dict(format=snapshot.FORMAT, itr=int(itr), rank=self.rank, world=self.world, first_env_id=env.first_env_id,
+                    num_envs=env.num_envs, model=env.model_name, precision=env.precision, seed=env.seed,
+                    state_r=env.state_r.cpu(), state_i=env.state_i.cpu(), fresh=bool(env._fresh),
+                    worker=self.workers[0].state_dict(), cpu_rng=torch.get_rng_state())
+
+    def restore(self, run_dir) -> int:
+        """Load the last complete snapshot of `run_dir` into this freshly built PPO and its environment and return the iteration
+        k it was taken at: `train(env_fn, n_itr, start_itr=k + 1)` then continues the run bit for bit.  A snapshot of another
+        world size, num_procs, env, precision, shard or format is refused with a SnapshotError before anything is loaded.
+        Runs make_optimizers() first if it has not run yet (it re-homes the parameters); captured graphs keep their addresses:
+        everything is copied in place."""
+        env = self._inner_env()
+        _, learner, shard = snapshot.load(run_dir, self.rank, self.world,
+                                          dict(env=env.model_name, precision=env.precision, num_procs=self.n_proc))
+        for key, mine in (("first_env_id", env.first_env_id), ("num_envs", env.num_envs), ("seed", env.seed)):
+            if shard.get(key) != mine:
+                raise SnapshotError(f"{key} mismatch: the rank-{self.rank} shard has {key}={shard.get(key)}, this run has {mine}")
+        if self.actor_optimizer is None:
+            self.make_optimizers()
+        a_opt, c_opt = self._fused_optimizers()
+        for name, have, want in (("flat_param", learner["flat_param"], self._flat_param), ("exp_avg", learner["exp_avg"], self._flat_m),
+                                 ("exp_avg_sq", learner["exp_avg_sq"], self._flat_v), ("state_r", shard["state_r"], env.state_r),
+                                 ("state_i", shard["state_i"], env.state_i)):
+            if have.shape != want.shape or have.dtype != want.dtype:
+                raise SnapshotError(f"{name} of the snapshot is {tuple(have.shape)} {have.dtype}, this run has "
+                                    f"{tuple(want.shape)} {want.dtype}")
+        with torch.no_grad():
+            self._flat_param.copy_(learner["flat_param"])
+            self._flat_m.copy_(learner["exp_avg"])
+            self._flat_v.copy_(learner["exp_avg_sq"])
+            for key, v in learner["obs_norm"].items():
+                net, name = key.split(".")
+                getattr(getattr(self, net), name).copy_(v)
+            env.state_r.copy_(shard["state_r"])
+            env.state_i.copy_(shard["state_i"])
+        env._fresh = bool(shard["fresh"])
+        a_opt.step_count, c_opt.step_count = learner["step_count"]
+        if self._comm is not None:
+            self._comm.set_step(learner["adam_step_dev"][0])
+        else:
+            a_opt.step_dev.fill_(learner["adam_step_dev"][0])
+            c_opt.step_dev.fill_(learner["adam_step_dev"][1])
+        self.workers[0].load_state_dict(shard["worker"])
+        self._best_eval, self.total_steps = learner["best_eval"], learner["total_steps"]
+        self._elapsed0 = learner["elapsed"]
+        self.iteration_count = learner["itr"]
+        torch.set_rng_state(shard["cpu_rng"])
+        torch.cuda.synchronize(self.device)
+        return learner["itr"]
 
     # ------------------------------------------------------------------ sampling (rl/algos/ppo.py:215-297)
     def sample_parallel_with_workers(self, deterministic=False) -> BatchData:
@@ -389,16 +474,18 @@ class PPO:
         return eval_batches, mean_rew, mean_len
 
     # ------------------------------------------------------------------ training loop (rl/algos/ppo.py:428-641)
-    def train(self, env_fn, n_itr, verbose=True):
+    def train(self, env_fn, n_itr, verbose=True, start_itr=0):
+        """Iterations start_itr .. n_itr - 1.  start_itr > 0 continues a run restored from its snapshot at start_itr - 1:
+        elapsed time and fps carry on, and the TensorBoard scalars the stopped run logged from start_itr on are dropped."""
         if self.actor_optimizer is None:
             self.make_optimizers()
         env = self.env
         obs_mirr = getattr(env, "mirror_clock_observation", None) if self.mirror_coeff else None
         act_mirr = getattr(env, "mirror_action", None) if self.mirror_coeff else None
-        train_start = time.time()
+        train_start = time.time() - getattr(self, "_elapsed0", 0.0)
         log = []
-        writer = self._tensorboard_writer() if self.rank == 0 else None
-        for itr in range(n_itr):
+        writer = self._tensorboard_writer(purge_step=start_itr or None) if self.rank == 0 else None
+        for itr in range(start_itr, n_itr):
             if verbose and self.rank == 0:
                 print(f"********** Iteration {itr} ************")
             self.policy.train()
@@ -468,14 +555,18 @@ class PPO:
                 if writer is not None:
                     writer.add_scalar("Eval/mean_reward", eval_rew, itr)
                     writer.add_scalar("Eval/mean_episode_length", eval_len, itr)
+                if getattr(self, "write_snapshots", False):      # after the evaluation batches: they advance the environments too
+                    if writer is not None:
+                        writer.flush()
+                    snapshot.write(self, itr, time.time() - train_start)
         if writer is not None:
             writer.flush()
             writer.close()
         return log
 
-    def _tensorboard_writer(self):
+    def _tensorboard_writer(self, purge_step=None):
         """TrainingLogger (rl/utils/logger.py:24-45): a SummaryWriter on the run directory; None if tensorboard is absent
-        or LHW_TENSORBOARD=0."""
+        or LHW_TENSORBOARD=0.  purge_step: a resumed run hides the events of steps >= purge_step from the earlier files."""
         import os
         if os.environ.get("LHW_TENSORBOARD", "1") == "0":
             return None
@@ -484,7 +575,7 @@ class PPO:
         except Exception:
             return None
         self.save_path.mkdir(parents=True, exist_ok=True)
-        return SummaryWriter(str(self.save_path), flush_secs=10)
+        return SummaryWriter(str(self.save_path), flush_secs=10, purge_step=purge_step)
 
     def save(self, itr):
         """actor_{itr}.pt / critic_{itr}.pt as whole pickled modules; itr None = the un-suffixed "best" pair

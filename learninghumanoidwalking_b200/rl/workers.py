@@ -33,6 +33,25 @@ class DeviceRolloutWorker:
         rollout buffers): call after anything that re-homes those tensors, e.g. PPO.make_optimizers()."""
         self._graphs = {}
 
+    def state_dict(self) -> dict:
+        """What the next sample() depends on besides the env's records and the networks (rl/snapshot.py)."""
+        cs = self.current_state
+        return dict(current_state=None if cs is None else cs.cpu(), gen=self.gen.get_state(), total_steps=int(self.total_steps))
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of state_dict(); in place where a captured graph may hold the address of current_state."""
+        cs = sd["current_state"]
+        if cs is None:
+            self.current_state = None
+        elif self.current_state is not None and self.current_state.shape == cs.shape:
+            self.current_state.copy_(cs)
+        else:
+            self.current_state = cs.to(self.device).clone()
+            self._noise = torch.zeros(0, cs.shape[0], self.env.act_dim, device=self.device)   # sample() sizes it
+            self._graphs = {}
+        self.gen.set_state(sd["gen"])
+        self.total_steps = int(sd["total_steps"])
+
     def sync_state(self, policy_state_dict=None, critic_state_dict=None, obs_mean=None, obs_std=None, iteration_count=0):
         """The learner and the sampler share the same modules on the same device: nothing to ship.  Kept so the
         call site of rl/algos/ppo.py:238-242 works unchanged; state dicts are loaded if given."""

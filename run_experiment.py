@@ -4,6 +4,7 @@
     python run_experiment.py train --env jvrc_walk --logdir /tmp/logs --num-procs 4096 --n-itr 100 --seed 0
     python -m torch.distributed.run --nproc-per-node 8 run_experiment.py train --env jvrc_step --num-procs 8192 ...
     python run_experiment.py eval --logdir /tmp/logs [--ep-len 10]
+    python run_experiment.py train ... --snapshot; python run_experiment.py resume --path RUN_DIR [--n-itr N]
 
 Same sub-commands and flags as the reference.  What differs underneath: `--num-procs` is the number of parallel environment
 copies (device resident, sharded by index across the ranks of a torchrun launch) instead of Ray worker processes; there is
@@ -49,7 +50,10 @@ TRAIN_FLAGS = [
     ("--minibatch-scale", dict(type=_S, default="auto", choices=["auto", "off"],
                                help="auto: --minibatch-size is scaled by (this rank's batch / 4800) so that an iteration keeps the reference's "
                                     "225 optimiser steps at its default flags; off: --minibatch-size samples per rank, literally")),
+    ("--snapshot", dict(action="store_true", help="at every checkpoint, also snapshot the whole training state for `resume`")),
 ]
+RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
+                ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
 EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P, default=None)),
               ("--out-dir", dict(type=_P, default=None, help="(videos are not produced by this build)")),
               ("--ep-len", dict(type=_I, default=10, help="seconds to play")), ("--seed", dict(type=_I, default=None))]
@@ -107,17 +111,10 @@ def _dist_setup():
     return 0, 1, 0
 
 
-def run_experiment(args):
-    from learninghumanoidwalking_b200.rl import PPO
+def make_env_fn(args, rank, world, local):
+    """This rank's shard of the `--num-procs` environments, wrapped in SymmetricEnv unless --no-mirror."""
     from learninghumanoidwalking_b200.rl.dist_utils import env_shard
     from learninghumanoidwalking_b200.rl.symmetric import SymmetricEnv
-    rank, world, local = _dist_setup()
-    timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
-    args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
-    if rank == 0:
-        print_system_info(args)
-    if args.recurrent or args.imitate:
-        raise NotImplementedError("--recurrent / --imitate are outside the accelerated path (SURVEY.md §2)")
     Env = import_env(args.env)
     if args.num_procs % world:
         raise SystemExit(f"--num-procs {args.num_procs} is not a multiple of the {world} ranks: every rank must hold the same number "
@@ -137,6 +134,25 @@ def run_experiment(args):
         except AttributeError as e:
             print("Warning! Cannot use SymmetricEnv.", e)
     _env.close()
+    return env_fn
+
+
+def run_experiment(args):
+    from learninghumanoidwalking_b200.rl import PPO
+    rank, world, local = _dist_setup()
+    timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
+    args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
+    if world > 1 and args.snapshot:
+        # every rank writes its shard of a snapshot into the run directory: rank 0's timestamp names it on all of them
+        import torch.distributed as dist
+        name = [args.logdir]
+        dist.broadcast_object_list(name, src=0)
+        args.logdir = name[0]
+    if rank == 0:
+        print_system_info(args)
+    if args.recurrent or args.imitate:
+        raise NotImplementedError("--recurrent / --imitate are outside the accelerated path (SURVEY.md §2)")
+    env_fn = make_env_fn(args, rank, world, local)
     if rank == 0:
         Path.mkdir(args.logdir, parents=True, exist_ok=True)
         with open(Path(args.logdir, "experiment.pkl"), "wb") as f:
@@ -152,6 +168,42 @@ def run_experiment(args):
         if rank == 0:
             print("Loaded (pre-trained) actor from: ", args.continued)
     algo.train(env_fn, args.n_itr, verbose=rank == 0)
+
+
+def resume(args):
+    """Continue the run in --path from its last snapshot (`train --snapshot`): the same run, bit for bit, as if it had never
+    stopped, up to --n-itr iterations in all (default: the run's own).  Checkpoints, TensorBoard events and snapshots go on
+    being written into the same directory.  Launch it with the same number of ranks as the run."""
+    from learninghumanoidwalking_b200.rl import PPO, snapshot
+    run_dir = Path(args.path)
+    try:
+        with open(run_dir / "experiment.pkl", "rb") as f:
+            run_args = pickle.load(f)
+    except FileNotFoundError:
+        raise SystemExit(f"resume: {run_dir} is not a run directory (no experiment.pkl)")
+    world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
+    try:    # refuse a snapshot this launch cannot continue before anything starts or is written
+        _, learner, _ = snapshot.load(run_dir, rank, world, dict(env=run_args.env, precision=run_args.precision,
+                                                                 num_procs=run_args.num_procs))
+    except snapshot.SnapshotError as e:
+        raise SystemExit(f"resume: {e}")
+    n_itr = args.n_itr if args.n_itr is not None else learner["args"]["n_itr"]
+    start = learner["itr"] + 1
+    if start >= n_itr:
+        if rank == 0:
+            print(f"Nothing to do: the snapshot of {run_dir} is at iteration {start - 1} of {n_itr}.")
+        return None
+    rank, world, local = _dist_setup()
+    run_args.logdir, run_args.n_itr, run_args.snapshot = run_dir, n_itr, True
+    if run_args.yaml is not None and Path(run_dir, Path(run_args.yaml).name).exists():
+        run_args.yaml = str(Path(run_dir, Path(run_args.yaml).name))     # the copy that rode along with the run
+    if rank == 0:
+        print_system_info(run_args)
+        print(f"Resuming {run_dir} after iteration {start - 1}.")
+    env_fn = make_env_fn(run_args, rank, world, local)
+    algo = PPO(env_fn, run_args, seed=run_args.seed)
+    algo.restore(run_dir)
+    return algo.train(env_fn, n_itr, verbose=rank == 0, start_itr=start)
 
 
 def evaluate(args):
@@ -213,8 +265,13 @@ def main(argv=None):
             parser.add_argument(flag, **kw)
         args = parser.parse_args(argv[1:])
         return evaluate(args)
+    elif argv and argv[0] == "resume":
+        for flag, kw in RESUME_FLAGS:
+            parser.add_argument(flag, **kw)
+        args = parser.parse_args(argv[1:])
+        return resume(args)
     else:
-        parser.error("usage: run_experiment.py {train,eval} ...")
+        parser.error("usage: run_experiment.py {train,eval,resume} ...")
 
 
 if __name__ == "__main__":
