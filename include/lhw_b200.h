@@ -79,6 +79,17 @@ int lhw_sim_bind(lhw_sim* sim, void* stream);
  * and passes it here; it takes effect at the next task reset.  No-op for the other variants. */
 int lhw_sim_set_step_height(lhw_sim* sim, double h);
 
+/* lhw_sim_render: replaces EvaluateEnv.run's frames (rl/utils/eval.py:37-86: mujoco.Renderer offscreen rendering of the
+ * roll-out into an mp4).  Ray-casts n_ids images of the environments env_ids[k] (device int32, each in [0, n_envs)) into
+ * rgb [n_ids, height, width, 3] uint8, row 0 at the top, in one launch; state_r / state_i are only read.  Drawn: every link
+ * as its equivalent-inertia box, the contact geometry of the feet, the slabs of jvrc_step / terrain, a checkerboard floor,
+ * one directional light with hard shadows (csrc/render_core.h has the scene and shading formulas).  Pinhole camera looking
+ * at (root_x + dx, root_y + dy, z) of each environment from `distance` metres, at `azimuth` / `elevation` (degrees,
+ * elevation > 0 looks down), vertical field of view `fovy` degrees.  width, height in 16..4096; distance > 0; fovy in (0, 180). */
+int lhw_sim_render(lhw_sim* sim, const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids,
+                   int width, int height, double dx, double dy, double z, double distance, double azimuth, double elevation,
+                   double fovy, uint8_t* rgb, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

@@ -30,6 +30,8 @@ SIGNATURES = {
                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lhw_sim_bind": (c_int, [c_void_p, c_void_p]),
     "lhw_sim_set_step_height": (c_int, [c_void_p, ctypes.c_double]),
+    "lhw_sim_render": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int] + [ctypes.c_double] * 7
+                       + [c_void_p, c_void_p]),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

@@ -22,10 +22,12 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "liblhw_b200.so")
 TORCH_LIB = os.path.join(PKG, "liblhw_b200_torch.so")     # csrc/torch_ops.cpp: the same entry points as torch.ops.lhw.*
 RECORD = os.path.join(PKG, "build_record.json")
-SOURCES = ["sim_kernels.cu", "ppo_kernels.cu", "comm_kernels.cu", "wgrad_kernels.cu"]
-HEADERS = ["sim_core.h", "model_pack.h", os.path.join("..", "..", "include", "lhw_b200.h"), "torch_ops.cpp"]
+SOURCES = ["sim_kernels.cu", "ppo_kernels.cu", "comm_kernels.cu", "wgrad_kernels.cu", "render_kernels.cu"]
+HEADERS = ["sim_core.h", "model_pack.h", "render_core.h", os.path.join("..", "..", "include", "lhw_b200.h"), "torch_ops.cpp"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
+# the renderer is built without FMA contraction, so that its images equal those of the host build of render_core.h
+SOURCE_FLAGS = {"render_kernels.cu": ["-fmad=false"]}
 
 
 def source_hashes() -> dict:
@@ -55,7 +57,8 @@ def needs_build() -> bool:
     if not os.path.exists(LIB) or not os.path.exists(TORCH_LIB):
         return True
     rec = read_record()
-    return rec is None or rec.get("sources") != source_hashes() or rec.get("flags") != NVCC_FLAGS
+    return (rec is None or rec.get("sources") != source_hashes() or rec.get("flags") != NVCC_FLAGS
+            or rec.get("source_flags") != SOURCE_FLAGS)
 
 
 def _sass_md5(nvcc: str, target: str = LIB) -> str | None:
@@ -102,7 +105,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     for src in SOURCES:
         obj = os.path.join(PKG, "build", src.replace(".cu", ".o"))
         objs.append(obj)
-        cmd = [nvcc] + NVCC_FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc] + NVCC_FLAGS + SOURCE_FLAGS.get(src, []) + ["-c", os.path.join(CSRC, src), "-o", obj]
         cmds.append(" ".join(cmd))
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     for src, p in procs:
@@ -118,7 +121,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     cmds.append(" ".join(link))
     cmds.append(" ".join(build_torch_ops(verbose)))
     ver = subprocess.run([nvcc, "--version"], capture_output=True, text=True).stdout.strip().splitlines()
-    json.dump(dict(library=os.path.basename(LIB), commands=cmds, flags=NVCC_FLAGS, nvcc=ver[-2:] if ver else None,
+    json.dump(dict(library=os.path.basename(LIB), commands=cmds, flags=NVCC_FLAGS, source_flags=SOURCE_FLAGS, nvcc=ver[-2:] if ver else None,
                    sources=source_hashes(), sass_md5=_sass_md5(nvcc),
                    step_kernel_sass_md5=_sass_md5(nvcc, os.path.join(PKG, "build", "sim_kernels.o")),
                    library_sha256=hashlib.sha256(open(LIB, "rb").read()).hexdigest(), host=platform.node(),

@@ -41,7 +41,7 @@
 
 #if defined(__CUDACC__) && !defined(LHW_CPU_EMU)
 #define LHW_DEV __device__ __forceinline__
-#define LHW_DEVNI __device__ __noinline__
+#define LHW_DEVNI inline __device__ __noinline__   // inline: the header is included by more than one translation unit
 #else
 #define LHW_DEV inline
 #define LHW_DEVNI inline

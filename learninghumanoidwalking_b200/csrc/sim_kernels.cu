@@ -17,6 +17,7 @@
 #include "../../include/lhw_b200.h"
 #define LHW_BLOCK_SYNC(on) do { if (on) __syncthreads(); } while (0)
 #include "model_pack.h"
+#include "render_core.h"
 
 using namespace lhw;
 
@@ -267,6 +268,14 @@ int launch_step(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_
   return 0;
 }
 
+// the renderer reads the sim's own global-memory model twin, whichever sim owns the constant bank
+template <class real, int NJ, int TK>
+int launch_render(lhw_sim* s, const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids, int width,
+                  int height, const render::Camera& cam, uint8_t* rgb, cudaStream_t st) {
+  return render_launch<real, NJ, TK>((const Model<real, NJ, TK>*)s->d_twin, (const real*)state_r, state_i, n_envs, env_ids, n_ids, width,
+                                     height, cam, rgb, st);
+}
+
 // (precision, NJ) dispatch
 #define LHW_DISPATCH(s, FN, ...)                                                                                          \
   ((s)->tk == 2 ? ((s)->precision == 64 ? FN<double, NJ_JVRC, 2>(__VA_ARGS__) : FN<float, NJ_JVRC, 2>(__VA_ARGS__))          \
@@ -392,6 +401,22 @@ int lhw_sim_step(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32
   if (upload_model(s, st)) return -10;
   LHW_DISPATCH(s, launch_step, s, state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs,
                term_obs, reward, rew_terms, done, ended, ep_len, ep_rew, st);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_render(lhw_sim* s, const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids, int width,
+                   int height, double dx, double dy, double z, double distance, double azimuth, double elevation, double fovy,
+                   uint8_t* rgb, void* stream) {
+  if (!s || !state_r || !state_i || !env_ids || !rgb) return fail(-1, "null argument");
+  if (n_envs <= 0 || n_ids <= 0 || n_ids > 65535) return fail(-2, "n_envs must be positive and n_ids in 1..65535");
+  if (width < 16 || width > 4096 || height < 16 || height > 4096) return fail(-2, "width and height must lie in 16..4096");
+  if (!(distance > 0) || !(fovy > 0 && fovy < 180)) return fail(-2, "distance must be positive and fovy in (0, 180) degrees");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (upload_model(s, st)) return -10;   // leaves the sim's current model in its twin
+  const render::Camera cam = render::make_camera(dx, dy, z, distance, azimuth, elevation, fovy, width, height);
+  LHW_DISPATCH(s, launch_render, s, state_r, state_i, n_envs, env_ids, n_ids, width, height, cam, rgb, st);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

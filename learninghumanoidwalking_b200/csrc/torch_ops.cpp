@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -80,6 +80,28 @@ void sim_step(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t
                   actions.data_ptr(), (int)max_traj_len, autoreset ? 1 : 0, obs.data_ptr(), term_obs ? term_obs->data_ptr() : nullptr,
                   reward.data_ptr(), rew_terms ? rew_terms->data_ptr() : nullptr, done.data_ptr<int32_t>(), ended.data_ptr<int32_t>(),
                   ep_len ? ep_len->data_ptr<int32_t>() : nullptr, ep_rew ? ep_rew->data_ptr() : nullptr, stream_of(state_r)), "lhw_sim_step");
+}
+
+void sim_render(int64_t sim, const Tensor& state_r, const Tensor& state_i, const Tensor& env_ids, int64_t width, int64_t height, double dx,
+                double dy, double z, double distance, double azimuth, double elevation, double fovy, Tensor rgb) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(width >= 16 && width <= 4096 && height >= 16 && height <= 4096, "lhw: width and height must lie in 16..4096, got ", width,
+              " x ", height);
+  TORCH_CHECK(distance > 0, "lhw: camera distance must be positive, got ", distance);
+  TORCH_CHECK(fovy > 0 && fovy < 180, "lhw: fovy must lie in (0, 180) degrees, got ", fovy);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  check_cuda(env_ids, "env_ids", at::kInt, I.device);
+  TORCH_CHECK(env_ids.dim() == 1 && env_ids.numel() >= 1 && env_ids.numel() <= 65535, "lhw: env_ids must be a 1-D tensor of 1..65535 ids");
+  const int64_t k = env_ids.numel();
+  check_cuda(rgb, "rgb", at::kByte, I.device); check_shape(rgb, "rgb", {k, height, width, 3});
+  TORCH_CHECK(n >= 1, "lhw: no environments");
+  TORCH_CHECK(env_ids.min().item<int32_t>() >= 0 && env_ids.max().item<int32_t>() < n, "lhw: env_ids must lie in [0, ", n, ")");
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_render(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, env_ids.data_ptr<int32_t>(), (int)k, (int)width, (int)height,
+                    dx, dy, z, distance, azimuth, elevation, fovy, rgb.data_ptr<uint8_t>(), stream_of(state_r)), "lhw_sim_render");
 }
 
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
@@ -233,6 +255,8 @@ TORCH_LIBRARY(lhw, m) {
   m.def("sim_step(int sim, Tensor(a!) state_r, Tensor(b!) state_i, int seed, int first_env_id, Tensor actions, int max_traj_len, "
         "bool autoreset, Tensor(c!) obs, Tensor(d!)? term_obs, Tensor(e!) reward, Tensor(f!)? rew_terms, Tensor(g!) done, Tensor(h!) ended, "
         "Tensor(i!)? ep_len, Tensor(j!)? ep_rew) -> ()");
+  m.def("sim_render(int sim, Tensor state_r, Tensor state_i, Tensor env_ids, int width, int height, float dx, float dy, float z, "
+        "float distance, float azimuth, float elevation, float fovy, Tensor(a!) rgb) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -256,6 +280,7 @@ TORCH_LIBRARY(lhw, m) {
 TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_reset", &sim_reset);
   m.impl("sim_step", &sim_step);
+  m.impl("sim_render", &sim_render);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

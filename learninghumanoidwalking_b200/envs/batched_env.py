@@ -202,6 +202,25 @@ class BatchedHumanoidEnv:
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().lhw_sim_bind(self._h, _lib.current_stream_ptr()), "lhw_sim_bind")
 
+    def render_rgb(self, env_ids=(0,), width: int = 640, height: int = 480) -> torch.Tensor:
+        """Pictures of environments env_ids as a device uint8 tensor [len(env_ids), height, width, 3] (RGB, row 0 at the top),
+        ray-cast in one launch from their current records, which are only read.  The tracking camera looks at each robot from
+        the side (from -y), 3 m away, 15 degrees down, with a 45 degree vertical field of view (include/lhw_b200.h:
+        lhw_sim_render).  What is drawn: csrc/render_core.h."""
+        ids = torch.as_tensor(env_ids, dtype=torch.int32).reshape(-1).to(self.device)
+        rgb = torch.empty(len(ids), height, width, 3, dtype=torch.uint8, device=self.device)
+        cam = (0.0, 0.0, 0.9 if self.model_name == "h1" else 0.8, 3.0, 90.0, 15.0, 45.0)   # dx dy z distance azimuth elevation fovy
+        if _lib.use_torch_ops():
+            _lib.ops().sim_render(self._h.value, self.state_r, self.state_i, ids, width, height, *cam, rgb)
+            return rgb
+        if len(ids) and not (0 <= int(ids.min()) and int(ids.max()) < self.num_envs):
+            raise ValueError(f"env_ids must lie in [0, {self.num_envs})")
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().lhw_sim_render(self._h, self.state_r.data_ptr(), self.state_i.data_ptr(), self.num_envs, ids.data_ptr(),
+                                                 len(ids), width, height, *cam, rgb.data_ptr(), _lib.current_stream_ptr()),
+                       "lhw_sim_render")
+        return rgb
+
     # ------------------------------------------------------------------ host API (numpy in / out, copies inside)
     def step_host(self, actions: np.ndarray, autoreset: bool = True):
         """Reference-facing batched call with HOST buffers: H2D actions, one launch, D2H obs/reward/done."""

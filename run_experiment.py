@@ -9,7 +9,9 @@
 Same sub-commands and flags as the reference.  What differs underneath: `--num-procs` is the number of parallel environment
 copies (device resident, sharded by index across the ranks of a torchrun launch) instead of Ray worker processes; there is
 no Ray, no MuJoCo and no viewer — `eval` rolls the saved actor out deterministically on one device environment and prints
-the per-term reward means (the reference's EvaluateEnv renders a video with MuJoCo's GL context, out of scope here).
+the per-term reward means; with `--out-dir DIR` it also writes the roll-out as `DIR/<actor file stem>.mp4`, one frame per
+control step, ray-cast on the GPU (BatchedHumanoidEnv.render_rgb: inertia boxes, contact geometry, slabs and floor, not
+the reference's meshes) and encoded with OpenCV, where the reference's EvaluateEnv uses MuJoCo's offscreen renderer.
 Artefacts keep the reference's names and format: `<logdir>/<timestamp>_<env>/experiment.pkl`, `actor_<itr>.pt`,
 `critic_<itr>.pt` (whole pickled modules, rl/utils/checkpointer.py:51-83).
 """
@@ -55,7 +57,8 @@ TRAIN_FLAGS = [
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
 EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P, default=None)),
-              ("--out-dir", dict(type=_P, default=None, help="(videos are not produced by this build)")),
+              ("--out-dir", dict(type=_P, default=None, help="write the roll-out as <out-dir>/<actor file stem>.mp4 "
+                                                               "(640x480 at 1/control_dt fps; needs OpenCV, the cv2 module)")),
               ("--ep-len", dict(type=_I, default=10, help="seconds to play")), ("--seed", dict(type=_I, default=None))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain")   # the last one is an extension (BASELINE configs[4])
 
@@ -225,15 +228,36 @@ def evaluate(args):
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
         run_args = pickle.load(f)
+    cv2 = None
+    if args.out_dir is not None:
+        try:
+            import cv2
+        except ImportError as e:
+            raise SystemExit(f"eval --out-dir writes the video with OpenCV, and the cv2 module could not be imported ({e}); "
+                             "install opencv-python or opencv-python-headless")
     policy = torch.load(path_to_actor, weights_only=False).cuda().eval()
     print_system_info(args, training=False)
     env = import_env(run_args.env)(1, precision=64, seed=args.seed or 0)
     obs = env.reset().float()
     n_steps = int(args.ep_len / env.dt)
+    video = None
+    if cv2 is not None:
+        args.out_dir.mkdir(parents=True, exist_ok=True)
+        video_path = args.out_dir / (path_to_actor.stem + ".mp4")
+        video = cv2.VideoWriter(str(video_path), cv2.VideoWriter_fourcc(*"mp4v"), 1.0 / env.dt, (640, 480))
+        if not video.isOpened():
+            raise SystemExit(f"eval --out-dir: OpenCV cannot write {video_path} with the mp4v codec")
+
+    def frame():
+        if video is not None:
+            video.write(env.render_rgb((0,), 640, 480)[0].flip(-1).cpu().numpy())   # RGB -> OpenCV's BGR
+
+    frame()
     totals, ep_ret, ep_len, episodes = torch.zeros(10, dtype=env.dtype, device=env.device), 0.0, 0, []
     with torch.no_grad():
         for _ in range(n_steps):
             obs, rew, done, _ = env.step(policy(obs, deterministic=True).to(env.dtype), autoreset=False)
+            frame()
             totals += env.rew_terms[0]
             ep_ret, ep_len = ep_ret + float(rew[0]), ep_len + 1
             if bool(done[0]):
@@ -245,6 +269,9 @@ def evaluate(args):
     print(f"{len(episodes)} episode(s) in {n_steps} control steps: " + ", ".join(f"len {l} return {r:.2f}" for l, r in episodes))
     for name, v in zip(env.reward_names, (totals / n_steps).tolist()):
         print(f"  mean {name:>20s} {v:.4f}")
+    if video is not None:
+        video.release()
+        print(f"Wrote {video_path} ({n_steps + 1} frames)")
     env.close()
     return episodes
 

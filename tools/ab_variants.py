@@ -52,7 +52,7 @@ def build():
         if src == "sim_kernels.cu":
             continue
         obj = os.path.join(VDIR, src.replace(".cu", ".o"))
-        subprocess.check_call([nvcc] + flags + ["-c", os.path.join(B.CSRC, src), "-o", obj])
+        subprocess.check_call([nvcc] + flags + B.SOURCE_FLAGS.get(src, []) + ["-c", os.path.join(B.CSRC, src), "-o", obj])
         shared.append(obj)
     procs = []
     for name, defs in BUILDS.items():
