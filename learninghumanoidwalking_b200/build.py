@@ -40,8 +40,9 @@ def source_hashes() -> dict:
 
 def step_kernel_sass_md5() -> str | None:
     """md5 of the device code (SASS) of the step / reset kernels as built: the key that ties an ncu capture to a build.  Host-side
-    edits of sim_kernels.cu do not move it; any change of the kernels does.  Read from the build record, None when there is
-    no record."""
+    edits of sim_kernels.cu move it only when they change the order in which the host code first instantiates the kernels (the
+    dump lists them in the reverse of that order); any change of the kernels moves it.  Read from the build record, None when
+    there is no record."""
     rec = read_record()
     return rec.get("step_kernel_sass_md5") if rec else None
 

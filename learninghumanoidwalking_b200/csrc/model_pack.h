@@ -8,15 +8,35 @@
 
 namespace lhw {
 
+// the compile-time variant that with_variant hands its callable
+template <class R, int J, int T> struct Variant {
+  using real = R;
+  static constexpr int NJ = J, TK = T;
+};
+
+// calls f(Variant<real, NJ, TK>{}) for the variant whose code is `code` (sim_core.h LHW_FOR_EACH_VARIANT), with real = double
+// at precision 64 and float otherwise.  Returns 0, or -1 without calling f when no variant has that code.
+template <class F> int with_variant(int code, int precision, F&& f) {
+#define LHW_VARIANT_CASE(J, T)                                                      \
+  if (code == variant_code(J, T)) {                                                 \
+    if (precision == 64) f(Variant<double, J, T>{}); else f(Variant<float, J, T>{}); \
+    return 0;                                                                       \
+  }
+  LHW_FOR_EACH_VARIANT(LHW_VARIANT_CASE)
+#undef LHW_VARIANT_CASE
+  return -1;
+}
+
 // returns 0 on success, negative on malformed input
-// the first word is NJ + 100 * TK (6: jvrc_walk, 5: h1, 106: jvrc_step).  `plan_table` (STEP only): caller-owned buffer of
-// MAXPLAN * PLAN_STRIDE reals that receives the footstep plans; the caller points m.plans at its device copy.
+// the first word is the variant's code (sim_core.h variant_code: 6 jvrc_walk, 5 h1, 106 jvrc_step, 206 jvrc_walk_terrain).
+// `plan_table` (STEP only): caller-owned buffer of MAXPLAN * PLAN_STRIDE reals that receives the footstep plans; the caller
+// points m.plans at its device copy.
 template <class real, int NJ, int TK> int fill_model(Model<real, NJ, TK>& m, const double* b, int n, real* plan_table = nullptr) {
   constexpr int NL = 1 + 2 * NJ, NV = 6 + 2 * NJ, NQ = NV + 1, NU = 2 * NJ;
   int p = 0;
   auto rd = [&]() -> double { return p < n ? b[p++] : (p++, 0.0); };
   memset(&m, 0, sizeof(m));
-  if ((int)rd() != NJ + 100 * TK) return -1;
+  if ((int)rd() != variant_code(NJ, TK)) return -1;
   for (int i = 0; i < NL; i++) {
     for (int k = 0; k < 3; k++) m.link_pos[i][k] = (real)rd();
     for (int k = 0; k < 9; k++) m.link_rot[i][k] = (real)rd();

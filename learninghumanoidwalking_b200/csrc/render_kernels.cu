@@ -67,14 +67,9 @@ int render_launch(const Model<real, NJ, TK>* d_model, const real* state_r, const
 #define LHW_RENDER_INSTANCE(R, J, T)                                                                                              \
   template int render_launch<R, J, T>(const Model<R, J, T>*, const R*, const int32_t*, int, const int32_t*, int, int, int,        \
                                       const render::Camera&, uint8_t*, cudaStream_t);
-LHW_RENDER_INSTANCE(double, 6, 0)
-LHW_RENDER_INSTANCE(float, 6, 0)
-LHW_RENDER_INSTANCE(double, 5, 0)
-LHW_RENDER_INSTANCE(float, 5, 0)
-LHW_RENDER_INSTANCE(double, 6, 1)
-LHW_RENDER_INSTANCE(float, 6, 1)
-LHW_RENDER_INSTANCE(double, 6, 2)
-LHW_RENDER_INSTANCE(float, 6, 2)
+#define LHW_RENDER_VARIANT(J, T) LHW_RENDER_INSTANCE(double, J, T) LHW_RENDER_INSTANCE(float, J, T)
+LHW_FOR_EACH_VARIANT(LHW_RENDER_VARIANT)
+#undef LHW_RENDER_VARIANT
 #undef LHW_RENDER_INSTANCE
 
 }  // namespace lhw

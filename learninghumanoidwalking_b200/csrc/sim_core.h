@@ -125,6 +125,10 @@ template <> struct Cfg<6, 2> {  // JVRC-1, WalkingTask on uneven / compliant ter
   static constexpr int CPF = 8, NPTS = 8;  // = the slabs of the stepping stones, re-posed like the reference's manip_hfield hook
   static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, STEP = false, SLABS = true, TERRAIN = true;
 };
+// every (NJ, TK) above, once: the host code instantiates, dispatches and keeps its books from this list
+#define LHW_FOR_EACH_VARIANT(X) X(6, 0) X(5, 0) X(6, 1) X(6, 2)
+// a variant's code, the first word of its flat model (model/loader.py): 6, 5, 106, 206
+constexpr int variant_code(int nj, int tk) { return nj + 100 * tk; }
 constexpr int NSLAB = 20;          // stepping stones per env (envs/jvrc/gen_xml.py:147-153)
 constexpr int NCORNER = 4;         // corner slots per foot (mjc_PlaneBox keeps at most 4)
 constexpr int MAXPLAN = 128, PLAN_STRIDE = 1 + 3 * NSLAB;   // footstep plan table: [len, (x y theta) * len]

@@ -7,6 +7,10 @@
 // is used.  The shipped launch puts 8 (fp64) / 14 (fp32) environments in a block that meets at one __syncthreads() per
 // physics substep: the warps then run the same region of a kernel that is far larger than the instruction cache
 // (DESIGN.md §4.1, findings 2 and 6); LHW_WARPS_PER_BLOCK=1 gives the original one-warp blocks that never wait.
+//
+// Every kernel is instantiated for each robot / task variant of sim_core.h's LHW_FOR_EACH_VARIANT at both precisions.  A sim
+// is one SimOf<real, NJ, TK>: lhw_sim_create picks it from the model's first word and precision (model_pack.h with_variant),
+// and the other entry points call it through lhw_sim's virtual functions.
 #include <cuda_runtime.h>
 #include <stdio.h>
 
@@ -23,49 +27,45 @@ using namespace lhw;
 
 namespace {
 
-// robot / task variants (sim_core.h Cfg<NJ, TK>): <6,0> JVRC-1 walking, <5,0> Unitree H1 standing, <6,1> JVRC-1 stepping
-constexpr int NJ_JVRC = 6, NJ_H1 = 5;
-__constant__ Model<double, NJ_JVRC, 0> c_model_d;
-__constant__ Model<float, NJ_JVRC, 0> c_model_f;
-__constant__ Model<double, NJ_H1, 0> c_model_d5;
-__constant__ Model<float, NJ_H1, 0> c_model_f5;
-__constant__ Model<double, NJ_JVRC, 1> c_model_ds;
-__constant__ Model<float, NJ_JVRC, 1> c_model_fs;
-__constant__ Model<double, NJ_JVRC, 2> c_model_dt;
-__constant__ Model<float, NJ_JVRC, 2> c_model_ft;
+// the constant-bank models, one per variant (sim_core.h LHW_FOR_EACH_VARIANT) and precision.  Named objects in this order:
+// their bank offsets are compiled into the kernels' LDC instructions
+constexpr int NJ_JVRC = 6;
+__constant__ Model<double, 6, 0> c_model_d;
+__constant__ Model<float, 6, 0> c_model_f;
+__constant__ Model<double, 5, 0> c_model_d5;
+__constant__ Model<float, 5, 0> c_model_f5;
+__constant__ Model<double, 6, 1> c_model_ds;
+__constant__ Model<float, 6, 1> c_model_fs;
+__constant__ Model<double, 6, 2> c_model_dt;
+__constant__ Model<float, 6, 2> c_model_ft;
 
-template <class real, int NJ, int TK> __device__ __forceinline__ const Model<real, NJ, TK>& cmodel();
-template <> __device__ __forceinline__ const Model<double, NJ_JVRC, 0>& cmodel<double, NJ_JVRC, 0>() { return c_model_d; }
-template <> __device__ __forceinline__ const Model<float, NJ_JVRC, 0>& cmodel<float, NJ_JVRC, 0>() { return c_model_f; }
-template <> __device__ __forceinline__ const Model<double, NJ_H1, 0>& cmodel<double, NJ_H1, 0>() { return c_model_d5; }
-template <> __device__ __forceinline__ const Model<float, NJ_H1, 0>& cmodel<float, NJ_H1, 0>() { return c_model_f5; }
-template <> __device__ __forceinline__ const Model<double, NJ_JVRC, 1>& cmodel<double, NJ_JVRC, 1>() { return c_model_ds; }
-template <> __device__ __forceinline__ const Model<float, NJ_JVRC, 1>& cmodel<float, NJ_JVRC, 1>() { return c_model_fs; }
-template <> __device__ __forceinline__ const Model<double, NJ_JVRC, 2>& cmodel<double, NJ_JVRC, 2>() { return c_model_dt; }
-template <> __device__ __forceinline__ const Model<float, NJ_JVRC, 2>& cmodel<float, NJ_JVRC, 2>() { return c_model_ft; }
+// the variant's constant-bank object: the kernels read their model from it, SimOf::bind uploads to it
+template <class real, int NJ, int TK> __host__ __device__ __forceinline__ const Model<real, NJ, TK>& cmodel() {
+  constexpr bool D = sizeof(real) == 8;
+  if constexpr (D && NJ == 6 && TK == 0) return c_model_d;
+  if constexpr (!D && NJ == 6 && TK == 0) return c_model_f;
+  if constexpr (D && NJ == 5 && TK == 0) return c_model_d5;
+  if constexpr (!D && NJ == 5 && TK == 0) return c_model_f5;
+  if constexpr (D && NJ == 6 && TK == 1) return c_model_ds;
+  if constexpr (!D && NJ == 6 && TK == 1) return c_model_fs;
+  if constexpr (D && NJ == 6 && TK == 2) return c_model_dt;
+  if constexpr (!D && NJ == 6 && TK == 2) return c_model_ft;
+}
 
 }  // namespace
 // tell sim_core.h's out-of-line routines where the model really lives (constant bank -> LDC with immediate offsets)
 namespace lhw {
-#define LHW_MODEL_HOME(R, J, T, OBJ)                                                                         \
-  template <> struct ModelHome<R, J, T> {                                                                   \
-    static __device__ __forceinline__ const Model<R, J, T>& get(const Model<R, J, T>&) { return OBJ; }        \
-  };
-LHW_MODEL_HOME(double, NJ_JVRC, 0, c_model_d)
-LHW_MODEL_HOME(float, NJ_JVRC, 0, c_model_f)
-LHW_MODEL_HOME(double, NJ_H1, 0, c_model_d5)
-LHW_MODEL_HOME(float, NJ_H1, 0, c_model_f5)
-LHW_MODEL_HOME(double, NJ_JVRC, 1, c_model_ds)
-LHW_MODEL_HOME(float, NJ_JVRC, 1, c_model_fs)
-LHW_MODEL_HOME(double, NJ_JVRC, 2, c_model_dt)
-LHW_MODEL_HOME(float, NJ_JVRC, 2, c_model_ft)
-#undef LHW_MODEL_HOME
+template <int NJ, int TK> struct ModelHome<double, NJ, TK> {
+  static __device__ __forceinline__ const Model<double, NJ, TK>& get(const Model<double, NJ, TK>&) { return cmodel<double, NJ, TK>(); }
+};
+template <int NJ, int TK> struct ModelHome<float, NJ, TK> {
+  static __device__ __forceinline__ const Model<float, NJ, TK>& get(const Model<float, NJ, TK>&) { return cmodel<float, NJ, TK>(); }
+};
 }  // namespace lhw
 namespace {
 
 thread_local std::string g_err;
 std::atomic<long long> g_launches{0};
-const void* g_owner[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // which sim's model sits in each constant-memory slot
 
 int fail(int code, const std::string& msg) {
   g_err = msg;
@@ -166,59 +166,24 @@ __global__ void __launch_bounds__(sizeof(real) == 8 ? LHW_X_REGCAP : 896, 1)
 
 }  // namespace
 
+// what every sim has, whichever its variant; SimOf<real, NJ, TK> holds its model and launches its kernels
 struct lhw_sim {
-  int precision, device, warps_per_block, sync_mode, nj, tk;
-  Model<double, NJ_JVRC, 0> md;
-  Model<float, NJ_JVRC, 0> mf;
-  Model<double, NJ_H1, 0> md5;
-  Model<float, NJ_H1, 0> mf5;
-  Model<double, NJ_JVRC, 1> mds;
-  Model<float, NJ_JVRC, 1> mfs;
-  Model<double, NJ_JVRC, 2> mdt;
-  Model<float, NJ_JVRC, 2> mft;
-  void* d_plans = nullptr;   // SteppingTask footstep plans in HBM ([MAXPLAN][PLAN_STRIDE] reals of the sim's precision)
-  void* d_twin = nullptr;    // the active model record once more, in global memory (lane-indexed tables are read from there)
+  int precision, device, warps_per_block, sync_mode;
   size_t work_bytes;
-  int state_reals, obs_dim;
+  int state_reals, obs_dim, act_dim;
+  virtual ~lhw_sim() = default;
+  virtual int bind(cudaStream_t st) = 0;
+  virtual void reset(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
+                     int fresh, void* obs, cudaStream_t st) = 0;
+  virtual void step(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
+                    int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
+                    int32_t* ended, int32_t* ep_len, void* ep_rew, cudaStream_t st) = 0;
+  virtual void render(const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids, int width,
+                      int height, const render::Camera& cam, uint8_t* rgb, cudaStream_t st) = 0;
+  virtual void set_step_height(double h) = 0;
 };
 
 namespace {
-
-// copy the model to global memory as well and leave its address in the record that goes to the constant bank
-template <class M> int upload_twin(lhw_sim* s, M& host, cudaStream_t st) {
-  if (!s->d_twin) CUDA_OK(cudaMalloc(&s->d_twin, sizeof(M)));
-  host.gm = (const M*)s->d_twin;
-  CUDA_OK(cudaMemcpyAsync(s->d_twin, &host, sizeof(M), cudaMemcpyHostToDevice, st));
-  return 0;
-}
-
-int upload_model(lhw_sim* s, cudaStream_t st) {
-  const int slot = (s->tk == 2 ? 6 : s->tk ? 4 : (s->nj == NJ_JVRC ? 0 : 2)) + (s->precision == 64 ? 0 : 1);
-  if (g_owner[slot] == s) return 0;
-  {
-    int rc = 0;
-    if (s->tk == 2) rc = s->precision == 64 ? upload_twin(s, s->mdt, st) : upload_twin(s, s->mft, st);
-    else if (s->tk) rc = s->precision == 64 ? upload_twin(s, s->mds, st) : upload_twin(s, s->mfs, st);
-    else if (s->nj == NJ_JVRC) rc = s->precision == 64 ? upload_twin(s, s->md, st) : upload_twin(s, s->mf, st);
-    else rc = s->precision == 64 ? upload_twin(s, s->md5, st) : upload_twin(s, s->mf5, st);
-    if (rc != 0) return rc;
-  }
-  if (s->tk == 2) {
-    if (s->precision == 64) CUDA_OK(cudaMemcpyToSymbolAsync(c_model_dt, &s->mdt, sizeof(s->mdt), 0, cudaMemcpyHostToDevice, st));
-    else CUDA_OK(cudaMemcpyToSymbolAsync(c_model_ft, &s->mft, sizeof(s->mft), 0, cudaMemcpyHostToDevice, st));
-  } else if (s->tk) {
-    if (s->precision == 64) CUDA_OK(cudaMemcpyToSymbolAsync(c_model_ds, &s->mds, sizeof(s->mds), 0, cudaMemcpyHostToDevice, st));
-    else CUDA_OK(cudaMemcpyToSymbolAsync(c_model_fs, &s->mfs, sizeof(s->mfs), 0, cudaMemcpyHostToDevice, st));
-  } else if (s->nj == NJ_JVRC) {
-    if (s->precision == 64) CUDA_OK(cudaMemcpyToSymbolAsync(c_model_d, &s->md, sizeof(s->md), 0, cudaMemcpyHostToDevice, st));
-    else CUDA_OK(cudaMemcpyToSymbolAsync(c_model_f, &s->mf, sizeof(s->mf), 0, cudaMemcpyHostToDevice, st));
-  } else {
-    if (s->precision == 64) CUDA_OK(cudaMemcpyToSymbolAsync(c_model_d5, &s->md5, sizeof(s->md5), 0, cudaMemcpyHostToDevice, st));
-    else CUDA_OK(cudaMemcpyToSymbolAsync(c_model_f5, &s->mf5, sizeof(s->mf5), 0, cudaMemcpyHostToDevice, st));
-  }
-  g_owner[slot] = s;
-  return 0;
-}
 
 template <class K> int prepare_kernel(K kernel, size_t smem) {
   CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -242,46 +207,89 @@ template <class real, int NJ, int TK> int prepare_variant(lhw_sim* s) {
   return 0;
 }
 
-template <class real, int NJ, int TK>
-int launch_reset(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
-                 const int32_t* mask, int fresh, void* obs, cudaStream_t st) {
-  reset_kernel<real, NJ, TK><<<n_envs, 32, s->work_bytes, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, mask, fresh,
-                                                           (real*)obs);
-  return 0;
-}
+template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
+  using M = Model<real, NJ, TK>;
+  static inline const lhw_sim* owner = nullptr;   // the sim whose model sits in cmodel<real, NJ, TK>() now
+  M model;
+  M* d_twin = nullptr;       // the model once more, in global memory (lane-indexed tables are read from there)
+  real* d_plans = nullptr;   // SteppingTask footstep plans in HBM ([MAXPLAN][PLAN_STRIDE])
 
-template <class real, int NJ, int TK>
-int launch_step(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
-                const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
-                void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, cudaStream_t st) {
-  const int wpb = s->warps_per_block, grid = (n_envs + wpb - 1) / wpb;
-  const size_t smem = s->work_bytes * wpb;
-  if (wpb > 1)
-    step_kernel_mw<real, NJ, TK><<<grid, wpb * 32, smem, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id,
-                                                          (const real*)actions, max_traj_len, autoreset, (real*)obs,
-                                                          (real*)term_obs, (real*)reward, (real*)rew_terms, done, ended,
-                                                          ep_len, (real*)ep_rew, s->sync_mode);
-  else
-    step_kernel<real, NJ, TK><<<grid, 32, smem, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id,
-                                                 (const real*)actions, max_traj_len, autoreset, (real*)obs, (real*)term_obs,
-                                                 (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew);
-  return 0;
-}
+  ~SimOf() override {
+    if (owner == this) owner = nullptr;
+    if (d_plans) cudaFree(d_plans);
+    if (d_twin) cudaFree(d_twin);
+  }
 
-// the renderer reads the sim's own global-memory model twin, whichever sim owns the constant bank
-template <class real, int NJ, int TK>
-int launch_render(lhw_sim* s, const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids, int width,
-                  int height, const render::Camera& cam, uint8_t* rgb, cudaStream_t st) {
-  return render_launch<real, NJ, TK>((const Model<real, NJ, TK>*)s->d_twin, (const real*)state_r, state_i, n_envs, env_ids, n_ids, width,
-                                     height, cam, rgb, st);
-}
+  int init(const double* flat, int n_flat, int dev) {
+    precision = sizeof(real) == 8 ? 64 : 32;
+    device = dev;
+    act_dim = 2 * NJ;
+    std::vector<real> plans(Cfg<NJ, TK>::STEP ? (size_t)MAXPLAN * PLAN_STRIDE : 0);
+    const int rc = fill_model(model, flat, n_flat, plans.data());
+    if (rc != 0) return fail(-4, "malformed model array (fill_model rc " + std::to_string(rc) + ")");
+    if constexpr (Cfg<NJ, TK>::STEP) {
+      // SteppingTask: the footstep plans go to HBM in the sim's precision; the model constants hold the device pointer
+      cudaError_t e = cudaMalloc(&d_plans, plans.size() * sizeof(real));
+      if (e == cudaSuccess) e = cudaMemcpy(d_plans, plans.data(), plans.size() * sizeof(real), cudaMemcpyHostToDevice);
+      if (e != cudaSuccess) return fail(-10, std::string("footstep plan upload: ") + cudaGetErrorString(e));
+      model.plans = d_plans;
+    }
+    const char* env_wpb = getenv("LHW_WARPS_PER_BLOCK");
+    // lock-step blocks of 8 (fp64) / 14 (fp32) warps, 2 blocks per SM: what the 64 K registers and 228 KB of shared memory of
+    // an H100 SM hold at the kernels' launch bounds (prepare_variant shrinks the block when the device has less)
+    warps_per_block = env_wpb ? atoi(env_wpb) : (sizeof(real) == 8 ? (NJ == NJ_JVRC && !TK ? 8 : 7) : 14);
+    const char* env_sync = getenv("LHW_BLOCK_SYNC_MODE");
+    sync_mode = env_sync ? atoi(env_sync) : 1;
+    if (warps_per_block < 1) warps_per_block = 1;
+    return prepare_variant<real, NJ, TK>(this);
+  }
 
-// (precision, NJ) dispatch
-#define LHW_DISPATCH(s, FN, ...)                                                                                          \
-  ((s)->tk == 2 ? ((s)->precision == 64 ? FN<double, NJ_JVRC, 2>(__VA_ARGS__) : FN<float, NJ_JVRC, 2>(__VA_ARGS__))          \
-   : (s)->tk ? ((s)->precision == 64 ? FN<double, NJ_JVRC, 1>(__VA_ARGS__) : FN<float, NJ_JVRC, 1>(__VA_ARGS__))             \
-   : (s)->nj == NJ_JVRC ? ((s)->precision == 64 ? FN<double, NJ_JVRC, 0>(__VA_ARGS__) : FN<float, NJ_JVRC, 0>(__VA_ARGS__)) \
-                        : ((s)->precision == 64 ? FN<double, NJ_H1, 0>(__VA_ARGS__) : FN<float, NJ_H1, 0>(__VA_ARGS__)))
+  // make this sim's model the one in the constant bank, and copy it to the twin as well
+  int bind(cudaStream_t st) override {
+    if (owner == this) return 0;
+    if (!d_twin) CUDA_OK(cudaMalloc(&d_twin, sizeof(M)));
+    model.gm = d_twin;
+    CUDA_OK(cudaMemcpyAsync(d_twin, &model, sizeof(M), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyToSymbolAsync(cmodel<real, NJ, TK>(), &model, sizeof(M), 0, cudaMemcpyHostToDevice, st));
+    owner = this;
+    return 0;
+  }
+
+  void reset(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask, int fresh,
+             void* obs, cudaStream_t st) override {
+    reset_kernel<real, NJ, TK><<<n_envs, 32, work_bytes, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, mask, fresh,
+                                                             (real*)obs);
+  }
+
+  void step(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
+            int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
+            int32_t* ended, int32_t* ep_len, void* ep_rew, cudaStream_t st) override {
+    const int wpb = warps_per_block, grid = (n_envs + wpb - 1) / wpb;
+    const size_t smem = work_bytes * wpb;
+    if (wpb > 1)
+      step_kernel_mw<real, NJ, TK><<<grid, wpb * 32, smem, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id,
+                                                            (const real*)actions, max_traj_len, autoreset, (real*)obs,
+                                                            (real*)term_obs, (real*)reward, (real*)rew_terms, done, ended,
+                                                            ep_len, (real*)ep_rew, sync_mode);
+    else
+      step_kernel<real, NJ, TK><<<grid, 32, smem, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id,
+                                                   (const real*)actions, max_traj_len, autoreset, (real*)obs, (real*)term_obs,
+                                                   (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew);
+  }
+
+  // the renderer reads the sim's own global-memory model twin, whichever sim owns the constant bank
+  void render(const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids, int width, int height,
+              const render::Camera& cam, uint8_t* rgb, cudaStream_t st) override {
+    render_launch<real, NJ, TK>(d_twin, (const real*)state_r, state_i, n_envs, env_ids, n_ids, width, height, cam, rgb, st);
+  }
+
+  void set_step_height(double h) override {
+    if constexpr (Cfg<NJ, TK>::STEP) {   // only the SteppingTask has a curriculum
+      model.step_height = (real)h;
+      if (owner == this) owner = nullptr;   // re-upload the constants at the next launch / lhw_sim_bind
+    }
+  }
+};
 
 }  // namespace
 
@@ -299,85 +307,43 @@ int lhw_sim_create(lhw_sim** out, const double* flat, int n_flat, int precision,
   CUDA_OK(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return fail(-3, "no such CUDA device");
   CUDA_OK(cudaSetDevice(device));
-  const int var = (int)flat[0], nj = var % 100, tk = var / 100;
-  if (var != NJ_JVRC && var != NJ_H1 && var != 100 + NJ_JVRC && var != 200 + NJ_JVRC)
-    return fail(-4, "unsupported robot / task variant " + std::to_string(var));
-  lhw_sim* s = new lhw_sim();
-  s->precision = precision;
-  s->device = device;
-  s->nj = nj;
-  s->tk = tk;
+  const int var = (int)flat[0];
+  lhw_sim* s = nullptr;
   int rc = 0;
-  if (tk == 2) {
-    rc = fill_model(s->mdt, flat, n_flat);
-    if (rc == 0) rc = fill_model(s->mft, flat, n_flat);
-  } else if (tk) {
-    // SteppingTask: the footstep plans go to HBM in the sim's precision; the model constants hold the device pointer
-    const size_t words = (size_t)MAXPLAN * PLAN_STRIDE;
-    std::vector<double> pd(words, 0.0);
-    std::vector<float> pf(words, 0.0f);
-    rc = fill_model(s->mds, flat, n_flat, pd.data());
-    if (rc == 0) rc = fill_model(s->mfs, flat, n_flat, pf.data());
-    if (rc == 0) {
-      const size_t bytes = words * (precision == 64 ? sizeof(double) : sizeof(float));
-      cudaError_t e = cudaMalloc(&s->d_plans, bytes);
-      if (e == cudaSuccess) e = cudaMemcpy(s->d_plans, precision == 64 ? (const void*)pd.data() : (const void*)pf.data(), bytes, cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) { delete s; return fail(-10, std::string("footstep plan upload: ") + cudaGetErrorString(e)); }
-      s->mds.plans = (const double*)s->d_plans;
-      s->mfs.plans = (const float*)s->d_plans;
-    }
-  } else {
-    rc = nj == NJ_JVRC ? fill_model(s->md, flat, n_flat) : fill_model(s->md5, flat, n_flat);
-    if (rc == 0) rc = nj == NJ_JVRC ? fill_model(s->mf, flat, n_flat) : fill_model(s->mf5, flat, n_flat);
-  }
-  if (rc != 0) {
-    delete s;
-    return fail(-4, "malformed model array (fill_model rc " + std::to_string(rc) + ")");
-  }
-  const char* env_wpb = getenv("LHW_WARPS_PER_BLOCK");
-  // lock-step blocks of 8 (fp64) / 14 (fp32) warps, 2 blocks per SM: what the 64 K registers and 228 KB of shared memory of
-  // an H100 SM hold at the kernels' launch bounds (prepare_variant shrinks the block when the device has less)
-  s->warps_per_block = env_wpb ? atoi(env_wpb) : (precision == 64 ? (nj == NJ_JVRC && !tk ? 8 : 7) : 14);
-  const char* env_sync = getenv("LHW_BLOCK_SYNC_MODE");
-  s->sync_mode = env_sync ? atoi(env_sync) : 1;
-  if (s->warps_per_block < 1) s->warps_per_block = 1;
-  rc = LHW_DISPATCH(s, prepare_variant, s);
+  const int unknown = with_variant(var, precision, [&](auto v) {
+    using V = decltype(v);
+    auto* sv = new SimOf<typename V::real, V::NJ, V::TK>();
+    s = sv;
+    rc = sv->init(flat, n_flat, device);
+  });
+  if (unknown) return fail(-4, "unsupported robot / task variant " + std::to_string(var));
   if (rc != 0) { delete s; return rc; }
   *out = s;
   return 0;
 }
 
 int lhw_sim_destroy(lhw_sim* s) {
-  if (!s) return 0;
-  for (int k = 0; k < 8; k++)
-    if (g_owner[k] == s) g_owner[k] = nullptr;
-  if (s->d_plans) cudaFree(s->d_plans);
-  if (s->d_twin) cudaFree(s->d_twin);
   delete s;
   return 0;
 }
 
 int lhw_sim_set_step_height(lhw_sim* s, double h) {
   if (!s) return fail(-1, "null argument");
-  if (s->tk != 1) return 0;   // only the SteppingTask has a curriculum
-  s->mds.step_height = h;
-  s->mfs.step_height = (float)h;
-  for (int k = 4; k < 6; k++)
-    if (g_owner[k] == s) g_owner[k] = nullptr;   // re-upload the constants at the next launch / lhw_sim_bind
+  s->set_step_height(h);   // no-op but for the SteppingTask
   return 0;
 }
 
 int lhw_sim_state_reals(const lhw_sim* s) { return s ? s->state_reals : Dims<double, NJ_JVRC, 0>::NSTATE_R; }
 int lhw_sim_state_ints(const lhw_sim*) { return NSTATE_I; }
 int lhw_sim_obs_dim(const lhw_sim* s) { return s ? s->obs_dim : Dims<double, NJ_JVRC, 0>::NOBS; }
-int lhw_sim_act_dim(const lhw_sim* s) { return 2 * (s ? s->nj : NJ_JVRC); }
+int lhw_sim_act_dim(const lhw_sim* s) { return s ? s->act_dim : 2 * NJ_JVRC; }
 int lhw_sim_smem_bytes_per_env(const lhw_sim* s) { return (int)s->work_bytes; }
 int lhw_sim_precision(const lhw_sim* s) { return s ? s->precision : 0; }
 int lhw_sim_device(const lhw_sim* s) { return s ? s->device : -1; }
 
 int lhw_sim_bind(lhw_sim* s, void* stream) {
   if (!s) return fail(-1, "null argument");
-  return upload_model(s, (cudaStream_t)stream);
+  return s->bind((cudaStream_t)stream);
 }
 
 int lhw_sim_reset(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
@@ -385,8 +351,8 @@ int lhw_sim_reset(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint3
   if (!s || !state_r || !state_i) return fail(-1, "null argument");
   if (n_envs <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (upload_model(s, st)) return -10;
-  LHW_DISPATCH(s, launch_reset, s, state_r, state_i, n_envs, seed, first_env_id, mask, fresh, obs, st);
+  if (s->bind(st)) return -10;
+  s->reset(state_r, state_i, n_envs, seed, first_env_id, mask, fresh, obs, st);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -398,9 +364,9 @@ int lhw_sim_step(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32
   if (!s || !state_r || !state_i || !actions || !obs || !reward || !done || !ended) return fail(-1, "null argument");
   if (n_envs <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (upload_model(s, st)) return -10;
-  LHW_DISPATCH(s, launch_step, s, state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs,
-               term_obs, reward, rew_terms, done, ended, ep_len, ep_rew, st);
+  if (s->bind(st)) return -10;
+  s->step(state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs, term_obs, reward, rew_terms, done,
+          ended, ep_len, ep_rew, st);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -414,9 +380,9 @@ int lhw_sim_render(lhw_sim* s, const void* state_r, const int32_t* state_i, int 
   if (width < 16 || width > 4096 || height < 16 || height > 4096) return fail(-2, "width and height must lie in 16..4096");
   if (!(distance > 0) || !(fovy > 0 && fovy < 180)) return fail(-2, "distance must be positive and fovy in (0, 180) degrees");
   cudaStream_t st = (cudaStream_t)stream;
-  if (upload_model(s, st)) return -10;   // leaves the sim's current model in its twin
+  if (s->bind(st)) return -10;   // leaves the sim's current model in its twin
   const render::Camera cam = render::make_camera(dx, dy, z, distance, azimuth, elevation, fovy, width, height);
-  LHW_DISPATCH(s, launch_render, s, state_r, state_i, n_envs, env_ids, n_ids, width, height, cam, rgb, st);
+  s->render(state_r, state_i, n_envs, env_ids, n_ids, width, height, cam, rgb, st);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
