@@ -13,6 +13,7 @@
 //   JVRC stepping variant (Cfg<6,1>): envs/jvrc/jvrc_step.py:41-76, tasks/stepping_task.py:52-334 (footstep sequences,
 //   stepping-stone slabs, target tracking, goal-step observation), utils/footstep_plans.txt
 //   terrain extension (Cfg<6,2>): WalkingTask on re-posed terraces, ranges of tasks/walking_task.py:172-179 (not a reference env)
+//   H1 walking variant (Cfg<5,3>): the robot of Cfg<5,0> with the WalkingTask of Cfg<6,0> (envs/h1/h1_walk.py; DESIGN.md §4.6)
 //
 // Execution model.  Every phase is a `LHW_LANES(l) { ... }` block: on the GPU each of the 32 lanes of the
 // warp runs the body once with its own lane id and `LHW_SYNC()` is __syncwarp(); all inter-lane traffic goes
@@ -110,24 +111,30 @@ constexpr int MAXPAIR = 64;
 // flags, so each instantiation only carries its own code.
 template <int NJ, int TK> struct Cfg;
 template <> struct Cfg<6, 0> {  // JVRC-1, WalkingTask: box feet (mjc_PlaneBox: at most 4 of the 8 corners per foot)
-  static constexpr int CPF = 4, NPTS = 8;
-  static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, STEP = false, SLABS = false, TERRAIN = false;
+  static constexpr int CPF = 4, NPTS = 8, RFOOT = 0;
+  static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, H1OBS = false, STEP = false, SLABS = false, TERRAIN = false;
 };
 template <> struct Cfg<5, 0> {  // Unitree H1, StandingTask: 3 capsules per foot = 6 end spheres; dof friction loss;
-  static constexpr int CPF = 6, NPTS = 6;  // per-env randomised mass / com / damping / frictionloss; xfrc perturbations
-  static constexpr bool SPHERES = true, FLOSS = true, PERENV = true, STAND = true, STEP = false, SLABS = false, TERRAIN = false;
+  static constexpr int CPF = 6, NPTS = 6, RFOOT = 1;  // per-env randomised mass / com / damping / frictionloss; xfrc perturbations
+  static constexpr bool SPHERES = true, FLOSS = true, PERENV = true, STAND = true, H1OBS = true, STEP = false, SLABS = false, TERRAIN = false;
 };
 template <> struct Cfg<6, 1> {  // JVRC-1, SteppingTask: box feet on the floor + 20 per-env stepping-stone slabs;
-  static constexpr int CPF = 8, NPTS = 8;  // per foot 4 corner slots (with multiplicity) + 4 sole-edge x slab-boundary slots
-  static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, STEP = true, SLABS = true, TERRAIN = false;
+  static constexpr int CPF = 8, NPTS = 8, RFOOT = 0;  // per foot 4 corner slots (with multiplicity) + 4 sole-edge x slab-boundary slots
+  static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, H1OBS = false, STEP = true, SLABS = true, TERRAIN = false;
 };
 template <> struct Cfg<6, 2> {  // JVRC-1, WalkingTask on uneven / compliant terrain (extension, BASELINE configs[4]): 20 terraces
-  static constexpr int CPF = 8, NPTS = 8;  // = the slabs of the stepping stones, re-posed like the reference's manip_hfield hook
-  static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, STEP = false, SLABS = true, TERRAIN = true;
+  static constexpr int CPF = 8, NPTS = 8, RFOOT = 0;  // = the slabs of the stepping stones, re-posed like the reference's manip_hfield hook
+  static constexpr bool SPHERES = false, FLOSS = false, PERENV = false, STAND = false, H1OBS = false, STEP = false, SLABS = true, TERRAIN = true;
 };
+template <> struct Cfg<5, 3> {  // Unitree H1 (the robot of Cfg<5, 0>), WalkingTask (the task of Cfg<6, 0>)
+  static constexpr int CPF = 6, NPTS = 6, RFOOT = 1;
+  static constexpr bool SPHERES = true, FLOSS = true, PERENV = true, STAND = false, H1OBS = true, STEP = false, SLABS = false, TERRAIN = false;
+};
+// H1OBS: the observation starts with h1_base's robot state (+ motor torques) and carries uniform observation noise.
+// RFOOT: the chain that ends in the right foot (JVRC-1 lists its right leg first, H1 its left leg)
 // every (NJ, TK) above, once: the host code instantiates, dispatches and keeps its books from this list
-#define LHW_FOR_EACH_VARIANT(X) X(6, 0) X(5, 0) X(6, 1) X(6, 2)
-// a variant's code, the first word of its flat model (model/loader.py): 6, 5, 106, 206
+#define LHW_FOR_EACH_VARIANT(X) X(6, 0) X(5, 0) X(6, 1) X(6, 2) X(5, 3)
+// a variant's code, the first word of its flat model (model/loader.py): 6, 5, 106, 206, 305
 constexpr int variant_code(int nj, int tk) { return nj + 100 * tk; }
 constexpr int NSLAB = 20;          // stepping stones per env (envs/jvrc/gen_xml.py:147-153)
 constexpr int NCORNER = 4;         // corner slots per foot (mjc_PlaneBox keeps at most 4)
@@ -270,7 +277,9 @@ template <class real, int NJ, int TK> LHW_DEV const Model<real, NJ, TK>& model_r
 
 template <class real, int NJ, int TK> struct Dims {
   static constexpr int NL = 1 + 2 * NJ, NV = 6 + 2 * NJ, NQ = NV + 1, NU = 2 * NJ, NA = 6 + NJ;
-  static constexpr int NOBS = Cfg<NJ, TK>::STAND ? 5 + 3 * NU : (Cfg<NJ, TK>::STEP ? 5 + 2 * NU + 10 : 5 + 2 * NU + 8);
+  // robot state (roll, pitch, root angular velocity, joint positions / velocities [, motor torques]), then the task's words
+  static constexpr int NROBOT = Cfg<NJ, TK>::H1OBS ? 5 + 3 * NU : 5 + 2 * NU;
+  static constexpr int NOBS = NROBOT + (Cfg<NJ, TK>::STAND ? 0 : Cfg<NJ, TK>::STEP ? 10 : 8);
   // real-valued state record per env (HBM, env-major so one warp streams its env's record contiguously)
   static constexpr int NPARAM = Cfg<NJ, TK>::PERENV ? NL + 3 * NL + 6 + 2 * NU + 3 + 12 : (Cfg<NJ, TK>::SLABS ? 4 * NSLAB + 5 : 0);
   static constexpr int NSTATE_R = NQ + NV + NV + 5 * NU + 3 + 1 + NPARAM;
@@ -1736,7 +1745,7 @@ template <class real, int NJ, int TK> LHW_DEV void sample_ref(Work<real, NJ, TK>
 // observation (envs/jvrc/jvrc_base.py:133-145 + jvrc_walk.py:65-67): current qpos quat / qvel, LAGGED actuator state
 template <class real, int NJ, int TK> LHW_DEV void env_obs(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed) {
   (void)seed;
-  constexpr int NU = 2 * NJ;
+  constexpr int NU = 2 * NJ, NROBOT = Dims<real, NJ, TK>::NROBOT;
   LHW_LANES(l) {
     if (l == 0) {  // transforms3d quat2euler (sxyz) roll, pitch via quat2mat
       const real qw = w.qpos[3], x = w.qpos[4], y = w.qpos[5], z = w.qpos[6];
@@ -1756,27 +1765,27 @@ template <class real, int NJ, int TK> LHW_DEV void env_obs(Work<real, NJ, TK>& w
     } else if (!Cfg<NJ, TK>::STAND && l == 4) {
       real sn, cs;
       m_sincos((real)(2 * M_PI) * w.phase / m.period, &sn, &cs);
-      w.obs[5 + 2 * NU] = sn; w.obs[6 + 2 * NU] = cs;
+      w.obs[NROBOT] = sn; w.obs[NROBOT + 1] = cs;
     } else if (Cfg<NJ, TK>::STEP && l == 5) {
-      real* e = w.obs + 7 + 2 * NU;   // envs/jvrc/jvrc_step.py:67-76: goal steps x[2] y[2] z[2] theta[2]
+      real* e = w.obs + NROBOT + 2;   // envs/jvrc/jvrc_step.py:67-76: goal steps x[2] y[2] z[2] theta[2]
 #pragma unroll
       for (int i = 0; i < 8; i++) e[i] = w.goal[i];
     } else if (!Cfg<NJ, TK>::STAND && !Cfg<NJ, TK>::STEP && l == 5) {
-      real* e = w.obs + 7 + 2 * NU;
+      real* e = w.obs + NROBOT + 2;
       e[0] = w.mode == FORWARD; e[1] = w.mode == INPLACE; e[2] = w.mode == STANDING;
       e[3] = w.mode_ref[0]; e[4] = w.mode_ref[1]; e[5] = w.mode_ref[2];
     } else if (l >= 8 && l < 8 + NU) {
       w.obs[5 + l - 8] = w.act_len[l - 8];
       w.obs[5 + NU + l - 8] = w.act_vel[l - 8];
-      if constexpr (Cfg<NJ, TK>::STAND) w.obs[5 + 2 * NU + l - 8] = w.act_force[l - 8];   // motor torques (h1_base.py:97)
+      if constexpr (Cfg<NJ, TK>::H1OBS) w.obs[5 + 2 * NU + l - 8] = w.act_force[l - 8];   // motor torques (h1_base.py:97)
     }
   }
   LHW_SYNC();
-  if constexpr (Cfg<NJ, TK>::STAND) {
-    // uniform observation noise (base_humanoid_env.py:311-338): value i -> philox stream 40 + i/4, lane i%4
-    constexpr int NOBS = Dims<real, NJ, TK>::NOBS;
+  if constexpr (Cfg<NJ, TK>::H1OBS) {
+    // uniform observation noise (base_humanoid_env.py:311-338) on the robot state: value i -> philox stream 40 + i/4, lane i%4.
+    // The task's words after it (gait clock, mode, reference) are exact.
     LHW_LANES(l) {
-      for (int i = l; i < NOBS; i += 32) {
+      for (int i = l; i < NROBOT; i += 32) {
         const real sc = i < 2 ? m.obs_noise[0] : i < 5 ? m.obs_noise[1] : i < 5 + NU ? m.obs_noise[2]
                         : i < 5 + 2 * NU ? m.obs_noise[3] : m.obs_noise[4];
         if (sc > 0) {
@@ -2239,12 +2248,13 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
       else if (w.mode == INPLACE) { vx = vy = 0; }
       else { yaw_ref = 0; }
       const real PI4 = (real)(M_PI / 4);
+      constexpr int RF = Cfg<NJ, TK>::RFOOT, LF = 1 - RF;
       real r = 0;
       if (l == 0) {
-        const real nl = m_min(w.grf[1], m.fcap) / m.fcap * 2 - 1, nr = m_min(w.grf[0], m.fcap) / m.fcap * 2 - 1;
+        const real nl = m_min(w.grf[LF], m.fcap) / m.fcap * 2 - 1, nr = m_min(w.grf[RF], m.fcap) / m.fcap * 2 - 1;
         r = (real)0.225 * ((m_tan(PI4 * lfc * nl) + m_tan(PI4 * rfc * nr)) / 2);
       } else if (l == 1) {
-        const real lv = m_sqrt(dot3(w.foot_vel[1], w.foot_vel[1])), rv = m_sqrt(dot3(w.foot_vel[0], w.foot_vel[0]));
+        const real lv = m_sqrt(dot3(w.foot_vel[LF], w.foot_vel[LF])), rv = m_sqrt(dot3(w.foot_vel[RF], w.foot_vel[RF]));
         const real vl = m_min(lv, (real)0.2) / (real)0.2 * 2 - 1, vr = m_min(rv, (real)0.2) / (real)0.2 * 2 - 1;
         r = (real)0.225 * ((m_tan(PI4 * lvc * vl) + m_tan(PI4 * rvc * vr)) / 2);
       } else if (l == 2) {

@@ -39,6 +39,13 @@ __constant__ Model<float, 6, 1> c_model_fs;
 __constant__ Model<double, 6, 2> c_model_dt;
 __constant__ Model<float, 6, 2> c_model_ft;
 
+// H1 walking (5, 3) has no objects of its own: with them the ten models would need 66 896 of the bank's 65 536 bytes.  Its Model has the
+// layout of H1 standing's (5, 0) — the same NJ and foot points — so it borrows that variant's objects, and an h1 and an h1_walk
+// sim take turns in them as two sims of one variant do.
+template <int NJ, int TK> constexpr int bank_tk() { return NJ == 5 && TK == 3 ? 0 : TK; }
+static_assert(sizeof(Model<double, 5, 3>) == sizeof(Model<double, 5, 0>) && sizeof(Model<float, 5, 3>) == sizeof(Model<float, 5, 0>) &&
+              Cfg<5, 3>::NPTS == Cfg<5, 0>::NPTS, "h1_walk borrows h1's constant-bank objects: the Model layouts must agree");
+
 // the variant's constant-bank object: the kernels read their model from it, SimOf::bind uploads to it
 template <class real, int NJ, int TK> __host__ __device__ __forceinline__ const Model<real, NJ, TK>& cmodel() {
   constexpr bool D = sizeof(real) == 8;
@@ -50,6 +57,7 @@ template <class real, int NJ, int TK> __host__ __device__ __forceinline__ const 
   if constexpr (!D && NJ == 6 && TK == 1) return c_model_fs;
   if constexpr (D && NJ == 6 && TK == 2) return c_model_dt;
   if constexpr (!D && NJ == 6 && TK == 2) return c_model_ft;
+  if constexpr (NJ == 5 && TK == 3) return reinterpret_cast<const Model<real, 5, 3>&>(cmodel<real, 5, 0>());
 }
 
 }  // namespace
@@ -108,7 +116,7 @@ __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, i
 // access is [index + immediate] and no base register has to be kept (or rematerialised).  fp32: 28 blocks/SM (register
 // bound: 28 x 132 = 3696 environments at once on an H100, so a 4096-env batch is two waves); fp64: 16 blocks/SM (shared-memory bound).
 template <class real, int NJ, int TK>
-__global__ void __launch_bounds__(32, sizeof(real) == 4 ? (TK ? 24 : 28) : (TK ? 12 : (NJ == NJ_JVRC ? 16 : 15)))
+__global__ void __launch_bounds__(32, sizeof(real) == 4 ? (Cfg<NJ, TK>::SLABS ? 24 : 28) : (Cfg<NJ, TK>::SLABS ? 12 : (NJ == NJ_JVRC ? 16 : 15)))
     step_kernel(real* __restrict__ state_r, int32_t* __restrict__ state_i, int n_envs, uint32_t seed, uint32_t first_id,
                 const real* __restrict__ actions, int max_traj_len, int autoreset, real* __restrict__ obs,
                 real* __restrict__ term_obs, real* __restrict__ reward, real* __restrict__ rew_terms,
@@ -207,15 +215,19 @@ template <class real, int NJ, int TK> int prepare_variant(lhw_sim* s) {
   return 0;
 }
 
+// the sim whose model sits in a constant-bank object now, one record per object
+template <class real, int NJ, int BANK_TK> struct BankOwner { static inline const lhw_sim* sim = nullptr; };
+
 template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
   using M = Model<real, NJ, TK>;
-  static inline const lhw_sim* owner = nullptr;   // the sim whose model sits in cmodel<real, NJ, TK>() now
+  // the sim whose model sits in cmodel<real, NJ, TK>() now
+  static const lhw_sim*& owner() { return BankOwner<real, NJ, bank_tk<NJ, TK>()>::sim; }
   M model;
   M* d_twin = nullptr;       // the model once more, in global memory (lane-indexed tables are read from there)
   real* d_plans = nullptr;   // SteppingTask footstep plans in HBM ([MAXPLAN][PLAN_STRIDE])
 
   ~SimOf() override {
-    if (owner == this) owner = nullptr;
+    if (owner() == this) owner() = nullptr;
     if (d_plans) cudaFree(d_plans);
     if (d_twin) cudaFree(d_twin);
   }
@@ -246,12 +258,12 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
 
   // make this sim's model the one in the constant bank, and copy it to the twin as well
   int bind(cudaStream_t st) override {
-    if (owner == this) return 0;
+    if (owner() == this) return 0;
     if (!d_twin) CUDA_OK(cudaMalloc(&d_twin, sizeof(M)));
     model.gm = d_twin;
     CUDA_OK(cudaMemcpyAsync(d_twin, &model, sizeof(M), cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyToSymbolAsync(cmodel<real, NJ, TK>(), &model, sizeof(M), 0, cudaMemcpyHostToDevice, st));
-    owner = this;
+    owner() = this;
     return 0;
   }
 
@@ -286,7 +298,7 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
   void set_step_height(double h) override {
     if constexpr (Cfg<NJ, TK>::STEP) {   // only the SteppingTask has a curriculum
       model.step_height = (real)h;
-      if (owner == this) owner = nullptr;   // re-upload the constants at the next launch / lhw_sim_bind
+      if (owner() == this) owner() = nullptr;   // re-upload the constants at the next launch / lhw_sim_bind
     }
   }
 };

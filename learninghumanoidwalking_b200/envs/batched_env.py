@@ -25,6 +25,15 @@ STAND_REWARD_NAMES = ("com_vel_error", "yaw_vel_error", "height", "upperbody", "
 STEP_REWARD_NAMES = ("foot_frc_score", "foot_vel_score", "orient_cost", "height_error", "step_reward",
                      "upper_body_reward")                                                 # tasks/stepping_task.py:107-120
 N_REWARD_SLOTS = 10   # width of the kernel's reward-term record (csrc/sim_core.h NREW); unused slots are 0
+# h1_walk (DESIGN.md §4.6): joints (hip_yaw, hip_roll, hip_pitch, knee, ankle), left leg then right.  The mirror swaps the legs and
+# negates yaw and roll; in the observation also the root roll and the x, z angular velocities.  The 8 walking-task words map to
+# themselves, as in jvrc_walk.  -0.1 stands for "-0" (index 0 negated), as in the reference's lists.
+H1_WALK_MIRRORED_OBS = [-0.1, 1, -2, 3, -4,
+                        -10, -11, 12, 13, 14, -5, -6, 7, 8, 9,            # joint positions
+                        -20, -21, 22, 23, 24, -15, -16, 17, 18, 19,       # joint velocities
+                        -30, -31, 32, 33, 34, -25, -26, 27, 28, 29,       # motor torques
+                        35, 36, 37, 38, 39, 40, 41, 42]                   # clock sin / cos, mode one-hot, mode reference
+H1_WALK_MIRRORED_ACTS = [-5, -6, 7, 8, 9, -0.1, -1, 2, 3, 4]
 
 
 class _Robot(SimpleNamespace):
@@ -99,13 +108,21 @@ class BatchedHumanoidEnv:
     def _setup_reference_attributes(self, model: str, cfg: dict) -> None:
         """obs_mean / obs_std, reward names and the robot's mirror lists exactly as the reference env classes set them
         (pure numpy; pinned to the reference's own method bodies by tests/golden/env_attributes.json)."""
-        if model == "h1":
+        if model in ("h1", "h1_walk"):
             # envs/h1/h1_env.py:37-55 (normalisation), envs/h1/h1_base.py:66-76 ; no mirror lists on the H1 robot
             self.reward_names = STAND_REWARD_NAMES
             half = np.asarray(cfg["half_sitting_pose"], dtype=float)
             self.obs_mean = np.concatenate((np.zeros(5), half, np.zeros(10), np.zeros(10)))
             self.obs_std = np.concatenate(([0.2, 0.2, 1, 1, 1], 0.5 * np.ones(10), 4 * np.ones(10), 100 * np.ones(10)))
             self.robot = SimpleNamespace(iteration_count=np.inf)
+            if model == "h1":
+                return
+            # h1_walk: h1's 35 robot-state entries, then jvrc_walk's 8 walking-task words (clock, mode one-hot, reference)
+            self.reward_names = REWARD_NAMES
+            self.obs_mean = np.concatenate((self.obs_mean, [0, 0, 0.5, 0.5, 0.5, 0, 0, 0]))
+            self.obs_std = np.concatenate((self.obs_std, [1, 1, 1, 1, 1, 0.5, 0.5, 0.5]))
+            self.robot = _Robot(mirrored_obs=list(H1_WALK_MIRRORED_OBS), mirrored_acts=list(H1_WALK_MIRRORED_ACTS),
+                                clock_inds=[35, 36], iteration_count=self._iteration_count, _on_iteration=None)
             return
         self.reward_names = REWARD_NAMES
         half = np.deg2rad(cfg["half_sitting_pose_deg"])
@@ -209,7 +226,7 @@ class BatchedHumanoidEnv:
         lhw_sim_render).  What is drawn: csrc/render_core.h."""
         ids = torch.as_tensor(env_ids, dtype=torch.int32).reshape(-1).to(self.device)
         rgb = torch.empty(len(ids), height, width, 3, dtype=torch.uint8, device=self.device)
-        cam = (0.0, 0.0, 0.9 if self.model_name == "h1" else 0.8, 3.0, 90.0, 15.0, 45.0)   # dx dy z distance azimuth elevation fovy
+        cam = (0.0, 0.0, 0.9 if self.model_name in ("h1", "h1_walk") else 0.8, 3.0, 90.0, 15.0, 45.0)   # dx dy z distance azimuth elevation fovy
         if _lib.use_torch_ops():
             _lib.ops().sim_render(self._h.value, self.state_r, self.state_i, ids, width, height, *cam, rgb)
             return rgb

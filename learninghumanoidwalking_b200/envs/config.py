@@ -25,12 +25,13 @@ def apply_config(mj: dict, user: dict) -> dict:
     """A deep copy of the compiled model `mj` with `user` (a parsed YAML) applied; raises ValueError on what cannot be honoured."""
     mj = copy.deepcopy(mj)
     c = mj["cfg"]
-    stand = mj["name"] == "h1"
+    h1 = mj["name"] in ("h1", "h1_walk")     # the H1 robot: its MJCF keys, pose in radians, noise / push / randomisation blocks
+    stand = mj["name"] == "h1"               # the standing task: no gait clock, no task block
     user = dict(user)
     for k in _IGNORED:
         user.pop(k, None)
     for k, compiled in _STRUCTURAL.items():
-        if k in user and bool(user.pop(k)) != compiled and stand:
+        if k in user and bool(user.pop(k)) != compiled and h1:
             raise ValueError(f"YAML key {k!r} changes the generated MJCF; recompile the model constants with tools/compile_model.py")
     if "sim_dt" in user or "control_dt" in user:
         sim_dt, control_dt = float(user.pop("sim_dt", c["sim_dt"])), float(user.pop("control_dt", c["control_dt"]))
@@ -60,7 +61,7 @@ def apply_config(mj: dict, user: dict) -> dict:
         pose = [float(x) for x in user.pop("half_sitting_pose")]
         if len(pose) != nu:
             raise ValueError(f"half_sitting_pose needs {nu} entries")
-        if stand:       # radians, envs/h1/h1_base.py
+        if h1:          # radians, envs/h1/h1_base.py
             c["half_sitting_pose"] = pose
             c["nominal_qpos"] = c["nominal_qpos"][:7] + pose
         else:           # degrees, envs/jvrc/jvrc_base.py:55-60
@@ -79,8 +80,8 @@ def apply_config(mj: dict, user: dict) -> dict:
         c["init_noise_deg"] = float(user.pop("init_noise"))
     for blk in ("observation_noise", "perturbation", "dynamics_randomization"):
         if blk in user:
-            if not stand:
-                raise ValueError(f"{blk}: only the H1 environment implements it (as in the reference, envs/jvrc has none)")
+            if not h1:
+                raise ValueError(f"{blk}: only the H1 environments implement it (as in the reference, envs/jvrc has none)")
             new = user.pop(blk)
             if blk == "observation_noise" and new.get("type", "uniform") != "uniform":
                 raise ValueError("observation_noise.type: only 'uniform' is implemented on the device")

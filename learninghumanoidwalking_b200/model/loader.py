@@ -32,10 +32,14 @@ def pack_model(mj: dict, tolerance: float | None = None, max_iter: int | None = 
             i = 1 + c * nj + k
             assert links[i]["parent"] == (0 if k == 0 else i - 1), "links must be ordered root, chain0, chain1"
     assert {mj["rfoot_link"], mj["lfoot_link"]} == {nj, 2 * nj}
+    # which chain ends in the right foot is compiled into the kernel (csrc/sim_core.h Cfg::RFOOT): chain 0 for JVRC-1, 1 for H1
+    assert mj["rfoot_link"] == (2 * nj if mj["name"] in ("h1", "h1_walk") else nj)
+    h1 = mj["name"] in ("h1", "h1_walk")  # the Unitree H1 robot: capsule feet, noise, randomisation, pushes
     stand = mj["name"] == "h1"          # Unitree H1 + StandingTask (csrc/sim_core.h Cfg<5, 0>)
+    h1_walk = mj["name"] == "h1_walk"   # Unitree H1 + WalkingTask (csrc/sim_core.h Cfg<5, 3>)
     step = mj["name"] == "jvrc_step"    # JVRC-1 + SteppingTask (csrc/sim_core.h Cfg<6, 1>)
     terrain = mj.get("terrain")         # JVRC-1 + WalkingTask on terraces (extension; csrc/sim_core.h Cfg<6, 2>)
-    b: list[float] = [nj + (100 if step else 200 if terrain else 0)]
+    b: list[float] = [nj + (100 if step else 200 if terrain else 300 if h1_walk else 0)]
     for lk in links:
         b += lk["pos"]
         b += list(np.asarray(lk["rot"], dtype=float).reshape(-1))
@@ -53,7 +57,7 @@ def pack_model(mj: dict, tolerance: float | None = None, max_iter: int | None = 
             b += [j["armature"], j["damping"], lo, hi, mj["dof_invweight0"][d]]
     assert [g["link"] for g in mj["geoms"]] == [nj, 2 * nj], "one ground-contact geom set per foot, chain order"
     for g in mj["geoms"]:
-        assert g["type"] == ("spheres" if stand else "box")
+        assert g["type"] == ("spheres" if h1 else "box")
         b += g.get("pos", [0.0, 0.0, 0.0])
         b += g.get("size", [0.0, 0.0, 0.0])
         b.append(mj["link_invweight0"][g["link"]][0])
@@ -90,13 +94,13 @@ def pack_model(mj: dict, tolerance: float | None = None, max_iter: int | None = 
     for a_, b_ in pairs:
         b += [a_, b_]
     # task / robot variant tail
-    if stand:
+    if h1:
         ns = c["observation_noise"] if observation_noise else {"enabled": False}
         lvl = ns["multiplier"] if ns["enabled"] else 0.0
         scales = [lvl * ns["scales"][k] for k in ("root_orient", "root_ang_vel", "motor_pos", "motor_vel", "motor_tau")] \
             if ns["enabled"] else [0.0] * 5
         pert, dyn = c["perturbation"], c["dynamics_randomization"]
-        b += [0.9, 1.4] + scales            # tasks/standing_task.py:124-125
+        b += ([0.6, 1.4] if h1_walk else [0.9, 1.4]) + scales   # tasks/walking_task.py:192-193, tasks/standing_task.py:124-125
         b += [int(dyn["interval"] / c["control_dt"]) if dyn["enable"] and domain_randomization else 0,
               int(pert["interval"] / c["control_dt"]) if pert["enable"] and domain_randomization else 0,
               pert["force_magnitude"], pert["torque_magnitude"],

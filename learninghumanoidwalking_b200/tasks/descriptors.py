@@ -68,11 +68,16 @@ class WalkingTask(_DeviceTask):
         t = cfg["task"]
         self._goal_height_ref, self._total_duration = t["goal_height"], t["total_duration"]
         self._swing_duration, self._stance_duration = t["swing_duration"], t["stance_duration"]
-        self._neutral_pose = np.deg2rad(cfg["half_sitting_pose_deg"])
         self._neutral_foot_orient = np.array([1, 0, 0, 0])
         self._period = int(np.floor(2 * self._total_duration * (1 / self._control_dt)))        # tasks/walking_task.py:201
-        self._root_body_name, self._lfoot_body_name, self._rfoot_body_name, self._head_body_name = \
-            "PELVIS_S", "L_ANKLE_P_S", "R_ANKLE_P_S", "NECK_P_S"                              # envs/jvrc/jvrc_base.py:26-29
+        if env.model_name == "h1_walk":   # the H1 robot: pose in radians (envs/h1/h1_base.py), the bodies StandingTask names
+            self._neutral_pose = np.asarray(cfg["half_sitting_pose"], dtype=float)
+            self._root_body_name, self._lfoot_body_name, self._rfoot_body_name, self._head_body_name = \
+                "pelvis", "left_ankle_link", "right_ankle_link", "torso_link"
+        else:
+            self._neutral_pose = np.deg2rad(cfg["half_sitting_pose_deg"])
+            self._root_body_name, self._lfoot_body_name, self._rfoot_body_name, self._head_body_name = \
+                "PELVIS_S", "L_ANKLE_P_S", "R_ANKLE_P_S", "NECK_P_S"                          # envs/jvrc/jvrc_base.py:26-29
         self.manip_hfield = env.model_name == "jvrc_walk_terrain"
 
     @property
@@ -142,7 +147,8 @@ class DeviceRobotInterface:
 
 
 def make_task(env, index: int = 0) -> BaseTask:
-    return {"jvrc_walk": WalkingTask, "jvrc_walk_terrain": WalkingTask, "jvrc_step": SteppingTask, "h1": StandingTask}[env.model_name](env, index)
+    return {"jvrc_walk": WalkingTask, "jvrc_walk_terrain": WalkingTask, "jvrc_step": SteppingTask, "h1": StandingTask,
+            "h1_walk": WalkingTask}[env.model_name](env, index)
 
 
 def model_view(env) -> SimpleNamespace:

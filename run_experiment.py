@@ -60,7 +60,7 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
               ("--out-dir", dict(type=_P, default=None, help="write the roll-out as <out-dir>/<actor file stem>.mp4 "
                                                                "(640x480 at 1/control_dt fps; needs OpenCV, the cv2 module)")),
               ("--ep-len", dict(type=_I, default=10, help="seconds to play")), ("--seed", dict(type=_I, default=None))]
-ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain")   # the last one is an extension (BASELINE configs[4])
+ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 
 
 def print_system_info(args, training=True):
@@ -235,6 +235,8 @@ def evaluate(args):
         except ImportError as e:
             raise SystemExit(f"eval --out-dir writes the video with OpenCV, and the cv2 module could not be imported ({e}); "
                              "install opencv-python or opencv-python-headless")
+    from learninghumanoidwalking_b200.rl.policies import install_reference_aliases
+    install_reference_aliases()   # a checkpoint pickles the reference's module names; a fresh `eval` process has not imported them
     policy = torch.load(path_to_actor, weights_only=False).cuda().eval()
     print_system_info(args, training=False)
     env = import_env(run_args.env)(1, precision=64, seed=args.seed or 0)

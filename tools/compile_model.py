@@ -545,12 +545,40 @@ def compile_h1():
     return model
 
 
+# h1_walk: the H1 robot of h1.json with a WalkingTask.  The reference's envs/h1/h1_walk.py is not read here, so these values are
+# this build's choices (DESIGN.md §4.6): jvrc_walk's gait durations, the standing task's goal height (tasks/standing_task.py), and
+# the torso's centre of mass (on the torso welded to the pelvis, in the root-link frame) as the upper-body reward's head point
+H1_WALK_TASK = dict(goal_height=0.98, total_duration=1.1, swing_duration=0.75, stance_duration=0.35)
+
+
+def derive_h1_walk(h1: dict) -> dict:
+    """model/h1_walk.json from model/h1.json: the same robot plus a walking `task` block and `head_in_root`."""
+    hw = json.loads(json.dumps(h1))
+    hw["name"] = "h1_walk"
+    hw["head_in_root"] = list(h1["root_parts"]["torso_com"])
+    hw["cfg"]["task"] = dict(H1_WALK_TASK)
+    return hw
+
+
+def write_h1_walk(out: str) -> str:
+    h1 = json.load(open(os.path.join(out, "h1.json")))
+    path = os.path.join(out, "h1_walk.json")
+    with open(path, "w") as f:
+        json.dump(derive_h1_walk(h1), f, indent=1)
+    return path
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.path.join(os.path.dirname(__file__), "..",
                                                   "learninghumanoidwalking_b200", "model"))
+    ap.add_argument("--h1-walk-only", action="store_true",
+                    help="only derive h1_walk.json from the h1.json already in --out (needs no reference checkout)")
     args = ap.parse_args()
     os.makedirs(args.out, exist_ok=True)
+    if args.h1_walk_only:
+        print("wrote", write_h1_walk(args.out))
+        return
     m = compile_jvrc()
     path = os.path.join(args.out, "jvrc_walk.json")
     if os.path.exists(path):   # tools/fit_collision_proxies.py adds this block afterwards; keep it across recompiles
@@ -586,6 +614,7 @@ def main():
     for lk in h["links"]:
         print(f"  {lk['name']:22s} parent {lk['parent']:2d} mass {lk['mass']:.4f} com {np.round(lk['com'], 4)}")
     print("  foot points", np.round(h["geoms"][0]["points"], 4).tolist())
+    print("wrote", write_h1_walk(args.out))
 
 
 if __name__ == "__main__":

@@ -89,7 +89,7 @@ class EmulationBackend:
 
     def __init__(self, model, n, seed, first_id):
         sys.path[:0] = [p for p in (ROOT, os.path.join(ROOT, "tests", "emu")) if p not in sys.path]
-        from emu import Emu
+        from emu_variants import Emu    # every variant of the kernel source, h1_walk included
         from learninghumanoidwalking_b200.model import load_model, pack_model
         mj = load_model(model)
         f64, f32 = pack_model(mj), pack_model(mj, tolerance=F32_TOLERANCE)
