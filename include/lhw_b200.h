@@ -126,6 +126,14 @@ int lhw_ppo_loss_partial_words(int B);
 int lhw_ppo_loss(const float* mu, const float* old_mu, const float* act, const float* adv, const float* ret, const float* val,
                  const float* mirr_or_null, const float* stds, int B, int A, float clip, float mirror_coeff, float ent_coeff,
                  float* g_mu, float* g_mirr_or_null, float* g_val, double* partials, unsigned int* ticket, float* out8, void* stream);
+/* lhw_ppo_loss_imitation: lhw_ppo_loss plus the imitation term of a teacher policy (rl/algos/ppo.py:361-368): from the teacher's
+ * actions teacher_mu [B,A] and an optional per-sample mask [B] (NULL = all ones), out8[5] = imitation_loss = mean over B*A of
+ * mask_b (mu_bk - teacher_bk)^2, total (out8[7]) gains imitate_coeff * imitation_loss and g_mu its gradient.  Same partials,
+ * ticket and determinism as lhw_ppo_loss. */
+int lhw_ppo_loss_imitation(const float* mu, const float* old_mu, const float* act, const float* adv, const float* ret, const float* val,
+                           const float* mirr_or_null, const float* stds, const float* teacher_mu, const float* mask_or_null, int B,
+                           int A, float clip, float mirror_coeff, float ent_coeff, float imitate_coeff, float* g_mu,
+                           float* g_mirr_or_null, float* g_val, double* partials, unsigned int* ticket, float* out8, void* stream);
 
 /* lhw_linear_wgrad: what `loss.backward()` (rl/algos/ppo.py:389-392) does per Linear layer of the actor / critic MLPs
  * (rl/policies/actor.py:122-189, critic.py) for its parameters: gW [N,K] = gy [M,N]^T x [M,K] and gb [N] = column sums of gy

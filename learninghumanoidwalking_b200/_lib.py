@@ -42,6 +42,7 @@ SIGNATURES = {
     "lhw_adv_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_float, c_void_p]),
     "lhw_ppo_loss_partial_words": (c_int, [c_int]),
     "lhw_ppo_loss": (c_int, [c_void_p] * 8 + [c_int, c_int, c_float, c_float, c_float] + [c_void_p] * 7),
+    "lhw_ppo_loss_imitation": (c_int, [c_void_p] * 10 + [c_int, c_int, c_float, c_float, c_float, c_float] + [c_void_p] * 7),
     "lhw_gather_minibatch": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_void_p]),
     "lhw_grad_sumsq": (c_int, [c_void_p, c_void_p, c_ll, c_float, c_void_p]),
     "lhw_linear_wgrad_workspace_floats": (c_ll, [c_int, c_int, c_int]),

@@ -344,15 +344,20 @@ int lhw_clip_adam_dev(float* param, const float* grad, float* exp_avg, float* ex
 //   total = actor + mirror_coeff * mirror + ent_coeff * entropy_penalty + critic  w.r.t. the policy mean, the mirrored
 //   mean and the values.  torch autograd then only runs the three MLP backward passes (cuBLAS).  One thread per sample,
 //   per-block partial sums combined in block order by the last block (ticket) -> run-to-run deterministic.
+// IMIT = true adds the imitation term (DESIGN §7.2): imitation = mean over B*A of m_b (mu_bk - teacher_bk)^2 with the mask
+//   m_b (1 where `imask` is null), in the spare partial slot 5, and imitate_coeff * imitation in the total.  IMIT = false is the
+//   kernel without it, instruction for instruction (the imitation arguments come last, so the others keep their offsets).
 namespace {
-constexpr int LOSS_BLOCK = 256, LOSS_NS = 6;   // partial sums: surrogate, clipfrac, critic, kl, mirror, (spare)
+constexpr int LOSS_BLOCK = 256, LOSS_NS = 6;   // partial sums: surrogate, clipfrac, critic, kl, mirror, imitation
+template <bool IMIT>
 __global__ void __launch_bounds__(LOSS_BLOCK)
     ppo_loss_kernel(const float* __restrict__ mu, const float* __restrict__ old_mu, const float* __restrict__ act,
                     const float* __restrict__ adv, const float* __restrict__ ret, const float* __restrict__ val,
                     const float* __restrict__ mirr /* [B,A] mirrored actions or null */, const float* __restrict__ stds, int B, int A,
                     float clip, float mirror_coeff, float ent_coeff, float* __restrict__ g_mu, float* __restrict__ g_mirr,
                     float* __restrict__ g_val, double* __restrict__ partials, unsigned int* __restrict__ ticket,
-                    float* __restrict__ out7) {
+                    float* __restrict__ out7, const float* __restrict__ teacher /* [B,A] teacher actions (IMIT) */,
+                    const float* __restrict__ imask /* [B] mask or null (IMIT) */, float imitate_coeff) {
   __shared__ double sh[LOSS_NS][LOSS_BLOCK / 32];
   __shared__ int last;
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -380,6 +385,11 @@ __global__ void __launch_bounds__(LOSS_BLOCK)
     const bool inside = ratio >= 1.0f - clip && ratio <= 1.0f + clip;
     const float glp = (inside || cpi < cl) ? -invB * ratio * ad : 0.0f;
     g_val[b] = 2.0f * dv * invB;
+    float ci = 0.f, mb = 1.f;     // d imitate_coeff * imitation / d (mu - teacher) = ci * (mu - teacher)
+    if constexpr (IMIT) {
+      mb = imask ? imask[b] : 1.0f;
+      ci = imitate_coeff * 2.0f * mb * invBA;
+    }
     for (int k = 0; k < A; k++) {
       const float sd = stds[k];
       float g = glp * (a[k] - m[k]) / (sd * sd);
@@ -389,6 +399,11 @@ __global__ void __launch_bounds__(LOSS_BLOCK)
         const float gm = mirror_coeff * 2.0f * d * invBA;
         g += gm;
         g_mirr[(size_t)b * A + k] = -gm;
+      }
+      if constexpr (IMIT) {
+        const float d = m[k] - teacher[(size_t)b * A + k];
+        s[5] += (double)mb * ((double)d * d);
+        if (ci != 0.f) g += ci * d;     // a zero mask or coefficient leaves g exactly as the kernel without the term has it
       }
       g_mu[(size_t)b * A + k] = g;
     }
@@ -430,11 +445,27 @@ __global__ void __launch_bounds__(LOSS_BLOCK)
     out7[2] = critic;                   // critic_loss
     out7[3] = (float)(t[3] / B);        // approx_kl_div
     out7[4] = mirror;                   // mirror_loss
-    out7[5] = 0.f;                      // imitation_loss (outside the accelerated path)
+    const float imitation = IMIT ? (float)(t[5] / ((double)B * A)) : 0.f;
+    out7[5] = imitation;                // imitation_loss (0 without a teacher)
     out7[6] = (float)(t[1] / B);        // clip_fraction
-    out7[7] = actor + mirror_coeff * mirror + ent_coeff * (-ent) + critic;   // total
+    if constexpr (IMIT)
+      out7[7] = actor + mirror_coeff * mirror + imitate_coeff * imitation + ent_coeff * (-ent) + critic;   // total
+    else
+      out7[7] = actor + mirror_coeff * mirror + ent_coeff * (-ent) + critic;   // total
     *ticket = 0;
   }
+}
+
+template <bool IMIT>
+int launch_ppo_loss(const float* mu, const float* old_mu, const float* act, const float* adv, const float* ret, const float* val,
+                    const float* mirr, const float* stds, int B, int A, float clip, float mirror_coeff, float ent_coeff, float* g_mu,
+                    float* g_mirr, float* g_val, double* partials, unsigned int* ticket, float* out8, const float* teacher,
+                    const float* imask, float imitate_coeff, void* stream) {
+  ppo_loss_kernel<IMIT><<<(B + LOSS_BLOCK - 1) / LOSS_BLOCK, LOSS_BLOCK, 0, (cudaStream_t)stream>>>(
+      mu, old_mu, act, adv, ret, val, mirr, stds, B, A, clip, mirror_coeff, ent_coeff, g_mu, g_mirr, g_val, partials, ticket, out8,
+      teacher, imask, imitate_coeff);
+  KCHECK("ppo_loss_kernel");
+  return 0;
 }
 }  // namespace
 
@@ -446,9 +477,18 @@ extern "C" int lhw_ppo_loss(const float* mu, const float* old_mu, const float* a
                             void* stream) {
   if (B <= 0 || A <= 0) return 0;
   if (mirr_or_null && !g_mirr_or_null) { g_perr = "lhw_ppo_loss: mirrored actions without a gradient buffer"; return -1; }
-  ppo_loss_kernel<<<(B + LOSS_BLOCK - 1) / LOSS_BLOCK, LOSS_BLOCK, 0, (cudaStream_t)stream>>>(
-      mu, old_mu, act, adv, ret, val, mirr_or_null, stds, B, A, clip, mirror_coeff, ent_coeff, g_mu, g_mirr_or_null, g_val, partials,
-      ticket, out8);
-  KCHECK("ppo_loss_kernel");
-  return 0;
+  return launch_ppo_loss<false>(mu, old_mu, act, adv, ret, val, mirr_or_null, stds, B, A, clip, mirror_coeff, ent_coeff, g_mu,
+                                g_mirr_or_null, g_val, partials, ticket, out8, nullptr, nullptr, 0.f, stream);
+}
+
+extern "C" int lhw_ppo_loss_imitation(const float* mu, const float* old_mu, const float* act, const float* adv, const float* ret,
+                                      const float* val, const float* mirr_or_null, const float* stds, const float* teacher_mu,
+                                      const float* mask_or_null, int B, int A, float clip, float mirror_coeff, float ent_coeff,
+                                      float imitate_coeff, float* g_mu, float* g_mirr_or_null, float* g_val, double* partials,
+                                      unsigned int* ticket, float* out8, void* stream) {
+  if (B <= 0 || A <= 0) return 0;
+  if (mirr_or_null && !g_mirr_or_null) { g_perr = "lhw_ppo_loss_imitation: mirrored actions without a gradient buffer"; return -1; }
+  if (!teacher_mu) { g_perr = "lhw_ppo_loss_imitation: no teacher actions"; return -1; }
+  return launch_ppo_loss<true>(mu, old_mu, act, adv, ret, val, mirr_or_null, stds, B, A, clip, mirror_coeff, ent_coeff, g_mu,
+                               g_mirr_or_null, g_val, partials, ticket, out8, teacher_mu, mask_or_null, imitate_coeff, stream);
 }

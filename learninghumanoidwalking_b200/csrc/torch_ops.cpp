@@ -169,9 +169,10 @@ void gather_minibatch(const Tensor& obs, const Tensor& act, const Tensor& ret, c
                           adv_b.data_ptr<float>(), (int)B, (int)od, (int)ad, stream_of(obs)), "lhw_gather_minibatch");
 }
 
-void ppo_loss(const Tensor& mu, const Tensor& old_mu, const Tensor& act, const Tensor& adv, const Tensor& ret, const Tensor& val,
-              const OptTensor& mirr, const Tensor& stds, double clip, double mirror_coeff, double ent_coeff, Tensor g_mu,
-              const OptTensor& g_mirr, Tensor g_val, Tensor partials, Tensor ticket, Tensor out8) {
+// the checks of ppo_loss's tensors, shared with ppo_loss_imitation; returns the device
+int check_ppo_loss(const Tensor& mu, const Tensor& old_mu, const Tensor& act, const Tensor& adv, const Tensor& ret, const Tensor& val,
+                   const OptTensor& mirr, const Tensor& stds, const Tensor& g_mu, const OptTensor& g_mirr, const Tensor& g_val,
+                   const Tensor& partials, const Tensor& ticket, const Tensor& out8) {
   TORCH_CHECK(mu.dim() == 2, "lhw: mu must be [B, A]");
   const int64_t B = mu.size(0), A = mu.size(1);
   const int dev = mu.is_cuda() ? mu.get_device() : -1;
@@ -187,12 +188,37 @@ void ppo_loss(const Tensor& mu, const Tensor& old_mu, const Tensor& act, const T
   check_cuda(partials, "partials", at::kDouble, dev); check_shape(partials, "partials", {lhw_ppo_loss_partial_words((int)B)});
   check_cuda(ticket, "ticket", at::kInt, dev); TORCH_CHECK(ticket.numel() >= 1, "lhw: ticket is empty");
   check_cuda(out8, "out8", at::kFloat, dev); check_shape(out8, "out8", {8});
+  return dev;
+}
+
+void ppo_loss(const Tensor& mu, const Tensor& old_mu, const Tensor& act, const Tensor& adv, const Tensor& ret, const Tensor& val,
+              const OptTensor& mirr, const Tensor& stds, double clip, double mirror_coeff, double ent_coeff, Tensor g_mu,
+              const OptTensor& g_mirr, Tensor g_val, Tensor partials, Tensor ticket, Tensor out8) {
+  const int dev = check_ppo_loss(mu, old_mu, act, adv, ret, val, mirr, stds, g_mu, g_mirr, g_val, partials, ticket, out8);
+  const int64_t B = mu.size(0), A = mu.size(1);
   c10::cuda::CUDAGuard guard(dev);
   ok(lhw_ppo_loss(mu.data_ptr<float>(), old_mu.data_ptr<float>(), act.data_ptr<float>(), adv.data_ptr<float>(), ret.data_ptr<float>(),
                   val.data_ptr<float>(), mirr ? mirr->data_ptr<float>() : nullptr, stds.data_ptr<float>(), (int)B, (int)A, (float)clip,
                   (float)mirror_coeff, (float)ent_coeff, g_mu.data_ptr<float>(), g_mirr ? g_mirr->data_ptr<float>() : nullptr,
                   g_val.data_ptr<float>(), partials.data_ptr<double>(), (unsigned int*)ticket.data_ptr<int>(), out8.data_ptr<float>(),
                   stream_of(mu)), "lhw_ppo_loss");
+}
+
+void ppo_loss_imitation(const Tensor& mu, const Tensor& old_mu, const Tensor& act, const Tensor& adv, const Tensor& ret, const Tensor& val,
+                        const OptTensor& mirr, const Tensor& stds, const Tensor& teacher_mu, const OptTensor& mask, double clip,
+                        double mirror_coeff, double ent_coeff, double imitate_coeff, Tensor g_mu, const OptTensor& g_mirr, Tensor g_val,
+                        Tensor partials, Tensor ticket, Tensor out8) {
+  const int dev = check_ppo_loss(mu, old_mu, act, adv, ret, val, mirr, stds, g_mu, g_mirr, g_val, partials, ticket, out8);
+  const int64_t B = mu.size(0), A = mu.size(1);
+  check_cuda(teacher_mu, "teacher_mu", at::kFloat, dev); check_shape(teacher_mu, "teacher_mu", {B, A});
+  if (mask) { check_cuda(*mask, "mask", at::kFloat, dev); TORCH_CHECK(mask->numel() == B, "lhw: mask must hold one value per sample"); }
+  c10::cuda::CUDAGuard guard(dev);
+  ok(lhw_ppo_loss_imitation(mu.data_ptr<float>(), old_mu.data_ptr<float>(), act.data_ptr<float>(), adv.data_ptr<float>(),
+                            ret.data_ptr<float>(), val.data_ptr<float>(), mirr ? mirr->data_ptr<float>() : nullptr, stds.data_ptr<float>(),
+                            teacher_mu.data_ptr<float>(), mask ? mask->data_ptr<float>() : nullptr, (int)B, (int)A, (float)clip,
+                            (float)mirror_coeff, (float)ent_coeff, (float)imitate_coeff, g_mu.data_ptr<float>(),
+                            g_mirr ? g_mirr->data_ptr<float>() : nullptr, g_val.data_ptr<float>(), partials.data_ptr<double>(),
+                            (unsigned int*)ticket.data_ptr<int>(), out8.data_ptr<float>(), stream_of(mu)), "lhw_ppo_loss_imitation");
 }
 
 void linear_wgrad(const Tensor& gy, const Tensor& x, Tensor gw, const OptTensor& gb, Tensor workspace) {
@@ -267,6 +293,9 @@ TORCH_LIBRARY(lhw, m) {
   m.def("ppo_loss(Tensor mu, Tensor old_mu, Tensor act, Tensor adv, Tensor ret, Tensor val, Tensor? mirr, Tensor stds, float clip, "
         "float mirror_coeff, float ent_coeff, Tensor(a!) g_mu, Tensor(b!)? g_mirr, Tensor(c!) g_val, Tensor(d!) partials, Tensor(e!) ticket, "
         "Tensor(f!) out8) -> ()");
+  m.def("ppo_loss_imitation(Tensor mu, Tensor old_mu, Tensor act, Tensor adv, Tensor ret, Tensor val, Tensor? mirr, Tensor stds, "
+        "Tensor teacher_mu, Tensor? mask, float clip, float mirror_coeff, float ent_coeff, float imitate_coeff, Tensor(a!) g_mu, "
+        "Tensor(b!)? g_mirr, Tensor(c!) g_val, Tensor(d!) partials, Tensor(e!) ticket, Tensor(f!) out8) -> ()");
   m.def("linear_wgrad(Tensor gy, Tensor x, Tensor(a!) gw, Tensor(b!)? gb, Tensor(c!) workspace) -> ()");
   m.def("grad_sumsq(Tensor grad, Tensor(a!) norm, float grad_scale) -> ()");
   m.def("clip_adam_dev(Tensor(a!) param, Tensor grad, Tensor(b!) exp_avg, Tensor(c!) exp_avg_sq, Tensor norm, Tensor(d!) step_dev, float lr, "
@@ -287,6 +316,7 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("adv_apply", &adv_apply);
   m.impl("gather_minibatch", &gather_minibatch);
   m.impl("ppo_loss", &ppo_loss);
+  m.impl("ppo_loss_imitation", &ppo_loss_imitation);
   m.impl("linear_wgrad", &linear_wgrad);
   m.impl("grad_sumsq", &grad_sumsq);
   m.impl("clip_adam_dev", &clip_adam_dev);

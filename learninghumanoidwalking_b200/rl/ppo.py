@@ -37,17 +37,23 @@ class _FusedPPOLoss(torch.autograd.Function):
     to autograd, which then only runs the MLP backward passes (cuBLAS)."""
 
     @staticmethod
-    def forward(ctx, mu, values, mirr, old_mu, act, adv, ret, stds, clip, mirror_coeff, ent_coeff, bufs):
+    def forward(ctx, mu, values, mirr, old_mu, act, adv, ret, stds, clip, mirror_coeff, ent_coeff, bufs, imitation=None):
         g_mu, g_mirr, g_val, partials, ticket, out8 = bufs
-        _lib.ops().ppo_loss(mu, old_mu, act, adv, ret, values, mirr, stds, clip, mirror_coeff, ent_coeff, g_mu,
-                            g_mirr if mirr is not None else None, g_val, partials, ticket, out8)
+        if imitation is None:
+            _lib.ops().ppo_loss(mu, old_mu, act, adv, ret, values, mirr, stds, clip, mirror_coeff, ent_coeff, g_mu,
+                                g_mirr if mirr is not None else None, g_val, partials, ticket, out8)
+        else:   # (teacher actions [B,A], mask [B,1] or None, imitate_coeff): the imitation term in the same launch
+            teacher_mu, imask, imitate_coeff = imitation
+            _lib.ops().ppo_loss_imitation(mu, old_mu, act, adv, ret, values, mirr, stds, teacher_mu, imask, clip, mirror_coeff,
+                                          ent_coeff, imitate_coeff, g_mu, g_mirr if mirr is not None else None, g_val, partials,
+                                          ticket, out8)
         ctx.bufs, ctx.has_mirr = (g_mu, g_mirr, g_val), mirr is not None
         return out8[7]
 
     @staticmethod
     def backward(ctx, gout):
         g_mu, g_mirr, g_val = ctx.bufs
-        return (g_mu * gout, g_val * gout, (g_mirr * gout) if ctx.has_mirr else None) + (None,) * 9
+        return (g_mu * gout, g_val * gout, (g_mirr * gout) if ctx.has_mirr else None) + (None,) * 10
 
 
 def get_worker_seed(master_seed: int, worker_id: int, offset: int = 0) -> int:
@@ -104,6 +110,12 @@ class PPO:
         self.critic = critic.to(self.device)
         self.old_policy = deepcopy(self.policy)
         self.base_policy, self.imitation_projector = None, None
+        if getattr(args, "imitate", None):
+            # the teacher (rl/imitation.py): every rank holds its own frozen copy; its parameters stay out of the flat buffer
+            from . import imitation
+            teacher, self.imitate_env, self.imitation_projector = imitation.check_teacher(
+                args.imitate, self._inner_env().model_name, getattr(args, "imitate_env", None))
+            self.base_policy = imitation.to_device(teacher, self.device)
         self.env_fn = env_fn
         wseed = get_worker_seed(seed if seed is not None else 0, self.rank)
         self.workers = [DeviceRolloutWorker(env, self.policy, self.critic, seed=wseed, worker_id=self.rank)]
@@ -238,7 +250,8 @@ class PPO:
     def _fused_loss_ok(self, obs_batch, mask) -> bool:
         import os
         return (os.environ.get("LHW_FUSED_LOSS", "1") != "0" and obs_batch.is_cuda and isinstance(mask, (int, float)) and mask == 1
-                and not getattr(self.policy, "learn_std", False) and self.imitate_coeff == 0.0 and isinstance(self.policy, Gaussian_FF_Actor))
+                and not getattr(self.policy, "learn_std", False) and isinstance(self.policy, Gaussian_FF_Actor)
+                and (self.imitate_coeff == 0.0 or getattr(self, "base_policy", None) is not None))
 
     def _loss_fused(self, obs_batch, action_batch, return_batch, advantage_batch, mirror_observation, mirror_action):
         """total loss (with the backward graph attached) and the 7 scalars, the elementwise part in one launch."""
@@ -259,12 +272,25 @@ class PPO:
             mu = self.policy(obs_batch, deterministic=True)
         with torch.no_grad():
             old_mu = self.old_policy(obs_batch, deterministic=True)
+        imitation = None
+        if getattr(self, "base_policy", None) is not None:
+            teacher_mu, imask = self._teacher_actions(obs_batch)
+            imitation = (teacher_mu.float().contiguous(), None if imask is None else imask.float().contiguous(), float(self.imitate_coeff))
         values = self.critic(obs_batch)
         stds = self.policy.stds if torch.is_tensor(self.policy.stds) else torch.as_tensor(self.policy.stds)
         total = _FusedPPOLoss.apply(mu, values, mirr, old_mu, action_batch, advantage_batch, return_batch,
-                                    stds.to(mu.device, torch.float32), float(self.clip), float(self.mirror_coeff), float(self.ent_coeff), bufs)
+                                    stds.to(mu.device, torch.float32), float(self.clip), float(self.mirror_coeff), float(self.ent_coeff), bufs,
+                                    imitation)
         out = bufs[5].clone()       # the buffer is rewritten by the next update; callers may hold on to the scalars
         return total, tuple(out[k] for k in range(7))
+
+    def _teacher_actions(self, obs_batch):
+        """(teacher actions, mask or None) for a minibatch, without a graph; both loss paths take them from here."""
+        if getattr(self, "imitation_projector", None) is None:
+            raise ValueError("imitation needs an imitation_projector that maps the student's observations to the teacher's")
+        with torch.no_grad():
+            teacher_obs, imask = self.imitation_projector(obs_batch)
+            return self.base_policy(teacher_obs, deterministic=True), imask
 
     def update_actor_critic(self, obs_batch, action_batch, return_batch, advantage_batch, mask,
                             mirror_observation=None, mirror_action=None):
@@ -290,7 +316,13 @@ class PPO:
             mirror_loss = (deterministic_actions - mirror_actions).pow(2).mean()
         else:
             mirror_loss = torch.zeros_like(actor_loss)
-        imitation_loss = torch.zeros_like(actor_loss)
+        if getattr(self, "base_policy", None) is not None:
+            # rl/algos/ppo.py:361-368: the teacher's deterministic actions on the projected observations (rl/imitation.py)
+            base_actions, imask = self._teacher_actions(obs_batch)
+            sq = (base_actions - deterministic_actions).pow(2)
+            imitation_loss = (sq if imask is None else sq * imask).mean()
+        else:
+            imitation_loss = torch.zeros_like(actor_loss)
         with torch.no_grad():
             approx_kl_div = torch.mean((ratio - 1) - (log_probs - old_log_probs))
         total_loss = (actor_loss + self.mirror_coeff * mirror_loss + self.imitate_coeff * imitation_loss

@@ -13,7 +13,8 @@ the per-term reward means; with `--out-dir DIR` it also writes the roll-out as `
 control step, ray-cast on the GPU (BatchedHumanoidEnv.render_rgb: inertia boxes, contact geometry, slabs and floor, not
 the reference's meshes) and encoded with OpenCV, where the reference's EvaluateEnv uses MuJoCo's offscreen renderer.
 Artefacts keep the reference's names and format: `<logdir>/<timestamp>_<env>/experiment.pkl`, `actor_<itr>.pt`,
-`critic_<itr>.pt` (whole pickled modules, rl/utils/checkpointer.py:51-83).
+`critic_<itr>.pt` (whole pickled modules, rl/utils/checkpointer.py:51-83); `train --imitate PATH` also keeps a copy of the
+teacher as `teacher.pt` (DESIGN §7.2).
 """
 import argparse
 import os
@@ -61,6 +62,7 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
                                                                "(640x480 at 1/control_dt fps; needs OpenCV, the cv2 module)")),
               ("--ep-len", dict(type=_I, default=10, help="seconds to play")), ("--seed", dict(type=_I, default=None))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
+from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
 
 def print_system_info(args, training=True):
@@ -153,16 +155,26 @@ def run_experiment(args):
         args.logdir = name[0]
     if rank == 0:
         print_system_info(args)
-    if args.recurrent or args.imitate:
-        raise NotImplementedError("--recurrent / --imitate are outside the accelerated path (SURVEY.md §2)")
+    if args.recurrent:
+        raise NotImplementedError("--recurrent is outside the accelerated path (SURVEY.md §2)")
+    if args.imitate:
+        # the teacher, its env and the projector to this env are checked before any environment or run directory exists
+        from learninghumanoidwalking_b200.rl import imitation
+        import_env(args.env)
+        try:
+            _, args.imitate_env, _ = imitation.check_teacher(args.imitate, args.env)
+        except ValueError as e:
+            raise SystemExit(f"train --imitate {args.imitate} for a {args.env} student: {e}")
     env_fn = make_env_fn(args, rank, world, local)
     if rank == 0:
+        import shutil
         Path.mkdir(args.logdir, parents=True, exist_ok=True)
         with open(Path(args.logdir, "experiment.pkl"), "wb") as f:
             pickle.dump(args, f)
         if args.yaml is not None:      # run_experiment.py:141-144: the YAML rides along with the run
-            import shutil
             shutil.copyfile(args.yaml, Path(args.logdir, Path(args.yaml).name))
+        if args.imitate:               # so does the teacher (not actor*.pt: `eval` and get_latest_actor glob that)
+            shutil.copyfile(args.imitate, Path(args.logdir, TEACHER_FILE))
     algo = PPO(env_fn, args, seed=args.seed)
     if args.continued is not None:
         actor = torch.load(args.continued, weights_only=False)
@@ -200,6 +212,8 @@ def resume(args):
     run_args.logdir, run_args.n_itr, run_args.snapshot = run_dir, n_itr, True
     if run_args.yaml is not None and Path(run_dir, Path(run_args.yaml).name).exists():
         run_args.yaml = str(Path(run_dir, Path(run_args.yaml).name))     # the copy that rode along with the run
+    if getattr(run_args, "imitate", None) and Path(run_dir, TEACHER_FILE).exists():
+        run_args.imitate = str(Path(run_dir, TEACHER_FILE))              # its env is run_args.imitate_env
     if rank == 0:
         print_system_info(run_args)
         print(f"Resuming {run_dir} after iteration {start - 1}.")

@@ -26,6 +26,10 @@ worker's buffer: GAE over every environment (gae64, vectorised over environments
 minibatch_indices call, gathers by plain indexing and all optimiser steps of S, free-running within the iteration.  A control
 repeats the float64 phase from parameters perturbed by fp32 rounding: free-running runs drift apart that far on their own.
 
+Imitation (opt-in, `--imitation`, IMITATION_CASES): the CUDA learner trains with a teacher (`train --imitate`, DESIGN §7.2),
+and S carries a float64 copy of the same teacher behind the same projector, so that its non-fused branch computes the
+reference's term (rl/algos/ppo.py:361-368).  Without a teacher S is the shadow above, unchanged.
+
 `python tools/learner_local_error.py` prints the distribution tables (needs a GPU); `--rehearse` runs the float64 parts on the
 CPU at a tiny size.
 """
@@ -35,6 +39,7 @@ import argparse
 import contextlib
 import os
 import sys
+import tempfile
 import time
 from copy import deepcopy
 from types import SimpleNamespace
@@ -91,7 +96,10 @@ class Shadow:
     """float64 policy, old policy and critic with hand-made torch Adam: the reference's optimiser sequence
     (rl/algos/ppo.py:389-396) through PPO.update_actor_critic's non-fused branch."""
 
-    def __init__(self, policy, old_policy, critic, hyper, sym=None, device="cpu", dtype=torch.float64):
+    def __init__(self, policy, old_policy, critic, hyper, sym=None, device="cpu", dtype=torch.float64, teacher=None,
+                 projector=None, imitate_coeff=0.0):
+        """teacher / projector / imitate_coeff: the imitation term (PPO.base_policy, .imitation_projector), with a copy of the
+        teacher in `dtype`; without a teacher the shadow has no imitation attributes at all, as before."""
         from learninghumanoidwalking_b200.rl.ppo import PPO
         self.dtype, self.device = dtype, torch.device(device)
         cast = lambda m: deepcopy(m).to(self.device, dtype)
@@ -102,6 +110,9 @@ class Shadow:
                                  ent_coeff=hyper["ent_coeff"], mirror_coeff=hyper["mirror_coeff"], imitate_coeff=0.0,
                                  grad_clip=hyper["max_grad_norm"], _comm=None, world=1,
                                  actor_optimizer=mk(self.policy), critic_optimizer=mk(self.critic))
+        if teacher is not None:
+            self.ppo.__dict__.update(base_policy=cast(teacher).eval().requires_grad_(False), imitation_projector=projector,
+                                     imitate_coeff=float(imitate_coeff))
         self.mirror = mirror_fns(sym, dtype, self.device)
 
     def params(self):
@@ -288,10 +299,34 @@ def choose_max_norm(norms, regime):
     return float(np.sqrt(lo.max() * hi.min()))
 
 
+def teacher_file(env):
+    """A saved actor for `--imitate`: the trained jvrc_walk actor of tests/golden (no experiment.pkl: the identity by width), or
+    for "h1" a 35-input actor with outputs of a trained policy's size, written next to an experiment.pkl naming h1 (the
+    h1 -> h1_walk projector)."""
+    if env == "jvrc_walk":
+        return os.path.join(ROOT, "tests", "golden", "trained_actor_jvrc_walk.pt")
+    assert env == "h1", env
+    import pickle
+    from learninghumanoidwalking_b200.rl.policies import Gaussian_FF_Actor, export_module
+    d = os.path.join(tempfile.gettempdir(), "lhw_learner_local_error", "h1_teacher")
+    os.makedirs(d, exist_ok=True)
+    g = torch.Generator().manual_seed(123)
+    actor = Gaussian_FF_Actor(35, 10)
+    with torch.no_grad():
+        for p in actor.parameters():
+            p.copy_(torch.randn(p.shape, generator=g) / p.shape[-1] ** 0.5 if p.dim() > 1 else torch.zeros(p.shape))
+    path = os.path.join(d, "actor_0.pt")
+    torch.save(export_module(actor), path)
+    with open(os.path.join(d, "experiment.pkl"), "wb") as f:
+        pickle.dump(SimpleNamespace(env="h1"), f)
+    return path
+
+
 def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, steps=7, regime="critic", learn_std=False,
-                  mirror=True, seed=0, hyper=None):
+                  mirror=True, seed=0, hyper=None, imitate=None, imitate_coeff=2.0):
     """Build the CUDA learner on a sampled batch of `model`, choose max_grad_norm for `regime`, run `steps` re-synchronised steps
     through _update_step (3 eager warm-ups, then the captured graph).  LHW_* switches come from the caller's environment.
+    imitate: the env of a teacher (teacher_file) to train with, at imitate_coeff; the shadows then carry its float64 copy.
     Returns (list of per-step error dicts, max_grad_norm)."""
     from learninghumanoidwalking_b200.envs import BatchedHumanoidEnv
     from learninghumanoidwalking_b200.rl import PPO
@@ -309,7 +344,11 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
                            minibatch_size=B, epochs=1, max_traj_len=400, num_procs=n_envs, max_grad_norm=0.5,
                            mirror_coeff=h["mirror_coeff"] if mirror else 0.0, std_dev=h["std_dev"], learn_std=learn_std,
                            steps_per_env=steps_per_env, eval_batches=0, eval_at_start=False, logdir="/tmp/lhw_learner_local_error")
+    if imitate is not None:
+        args.imitate, args.imitate_coeff = teacher_file(imitate), imitate_coeff
     ppo = PPO(env_fn, args, seed=seed)
+    teach = dict(teacher=ppo.base_policy, projector=ppo.imitation_projector, imitate_coeff=ppo.imitate_coeff) \
+        if imitate is not None else {}
     batch = ppo.sample_parallel_with_workers()
     obs, act = batch.states, batch.actions
     ret = batch.returns.contiguous()
@@ -321,7 +360,7 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
     old = deepcopy(ppo.policy)
     offset_mean_(old, seed)
     sym = sym_of(ppo.env)
-    probe = Shadow(ppo.policy, old, ppo.critic, hyper_of(ppo), sym, device=ppo.device)
+    probe = Shadow(ppo.policy, old, ppo.critic, hyper_of(ppo), sym, device=ppo.device, **teach)
     def first(cand, sh):
         i = cand[~sh.near_kink(obs[cand], act[cand])][:B]
         assert i.numel() == B, f"only {i.numel()} of {C} candidates are away from the loss's kinks"
@@ -330,8 +369,8 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
     ppo.grad_clip = choose_max_norm(norms, regime)
     ppo.make_optimizers()
     offset_mean_(ppo.old_policy, seed)
-    sh = Shadow(ppo.policy, ppo.old_policy, ppo.critic, hyper_of(ppo), sym, device=ppo.device)
-    sh_opt = Shadow(ppo.policy, ppo.old_policy, ppo.critic, hyper_of(ppo), sym, device=ppo.device)
+    sh = Shadow(ppo.policy, ppo.old_policy, ppo.critic, hyper_of(ppo), sym, device=ppo.device, **teach)
+    sh_opt = Shadow(ppo.policy, ppo.old_policy, ppo.critic, hyper_of(ppo), sym, device=ppo.device, **teach)
     obs_mirr = getattr(ppo.env, "mirror_clock_observation", None) if mirror else None
     act_mirr = getattr(ppo.env, "mirror_action", None) if mirror else None
     res = []
@@ -344,6 +383,8 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
         ob, ab, rb, db = ppo.gather_minibatch(obs, act, ret, (adv * s).contiguous(), i)
         e = compare_step(ppo, sh, sh_opt, ob, ab, rb, db, obs_mirr, act_mirr)
         e["graph"], e["B"], e["skipped"] = ppo._ug is not None, ob.shape[0], int(sh.near_kink(obs[cand], act[cand]).sum())
+        if imitate is not None:   # the minibatch's taught samples (the projector's mask; all of them without one)
+            e["taught"] = B if ppo.imitation_projector(ob)[1] is None else int(ppo.imitation_projector(ob)[1].sum())
         res.append(e)
     ppo.env.close()
     return res, ppo.grad_clip
@@ -504,6 +545,13 @@ CASES = {
 }
 
 
+# opt-in (--imitation): the learner with a teacher, the jvrc_walk identity pair and h1 -> h1_walk (the standing projector)
+IMITATION_CASES = {
+    "imitate_jvrc_walk_B21845": (dict(model="jvrc_walk", B=21845, regime="both", imitate="jvrc_walk"), {}),
+    "imitate_h1_to_h1_walk_B21845": (dict(model="h1_walk", B=21845, regime="neither", imitate="h1"), {}),
+}
+
+
 @contextlib.contextmanager
 def switches(env):
     old = {k: os.environ.get(k) for k in env}
@@ -550,14 +598,16 @@ def main():
     ap.add_argument("--rehearse", action="store_true", help="the float64 parts on the CPU at a tiny size")
     ap.add_argument("--cases", default=",".join(CASES))
     ap.add_argument("--iterations", default="jvrc_walk,h1", help="whole-iteration tier variants ('' skips it)")
+    ap.add_argument("--imitation", action="store_true", help="also the per-step cases with a teacher (IMITATION_CASES)")
     args = ap.parse_args()
     if args.rehearse:
         print(rehearse())
         return
     print("| case | quantity | median | p99 | max | bound |\n|---|---|---|---|---|---|")
     notes = []
-    for name in [c for c in args.cases.split(",") if c]:
-        kw, env = CASES[name]
+    names = [c for c in args.cases.split(",") if c] + (list(IMITATION_CASES) if args.imitation else [])
+    for name in names:
+        kw, env = {**CASES, **IMITATION_CASES}[name]
         t0 = time.time()
         with switches(env):
             res, mn = per_step_case(**kw)
