@@ -192,6 +192,20 @@ int lhw_fused_allreduce_clip_adam(lhw_comm* comm, float* param, float* exp_avg, 
                                   void* stream);
 int lhw_comm_status(lhw_comm* comm, int* error_word, int* adam_steps, float* norms2, void* stream);
 int lhw_comm_set_step(lhw_comm* comm, int adam_steps, void* stream);
+/* KL-adaptive learning rate (rsl_rl's schedule, DESIGN.md §7.3), the same three launches otherwise.  Each rank publishes its
+ * minibatch KL (kl: one device float, e.g. the loss's approx_kl_div) in its comm block after the flag words; once every peer
+ * is ready, K1 takes the rank-order float64 mean of the W KL words and updates the float64 rate lr_dev[0] (device memory):
+ * mean > 2 desired_kl -> lr = max(1e-5, lr / 1.5); 0 < mean < desired_kl / 2 -> lr = min(1e-2, lr * 1.5); otherwise (NaN
+ * included) unchanged.  Adam then uses (float)lr_dev[0] in the same step.  Every rank computes the same bits, and the
+ * launches stay graph-capturable: the rate is never a by-value argument.  desired_kl > 0.
+ * lhw_comm_lr_ptr: the comm's own float64 rate word (the host passes it as lr_dev); lhw_comm_get_lr / lhw_comm_set_lr read
+ * and write it (logging, resume) and synchronise `stream`; set_lr needs lr > 0. */
+int lhw_fused_allreduce_clip_adam_adaptive(lhw_comm* comm, float* param, float* exp_avg, float* exp_avg_sq, long long n_actor,
+                                           long long n_total, const float* kl, double* lr_dev, double desired_kl, float beta1,
+                                           float beta2, float eps, float max_norm, void* stream);
+double* lhw_comm_lr_ptr(lhw_comm* comm);
+int lhw_comm_get_lr(lhw_comm* comm, double* lr_host, void* stream);
+int lhw_comm_set_lr(lhw_comm* comm, double lr, void* stream);
 
 #ifdef __cplusplus
 }

@@ -60,6 +60,11 @@ SIGNATURES = {
                                               c_float, c_float, c_float, c_void_p]),
     "lhw_comm_status": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lhw_comm_set_step": (c_int, [c_void_p, c_int, c_void_p]),
+    "lhw_fused_allreduce_clip_adam_adaptive": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_void_p,
+                                                       ctypes.c_double, c_float, c_float, c_float, c_float, c_void_p]),
+    "lhw_comm_lr_ptr": (c_void_p, [c_void_p]),
+    "lhw_comm_get_lr": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "lhw_comm_set_lr": (c_int, [c_void_p, ctypes.c_double, c_void_p]),
     "lhw_clip_adam_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_float, c_float, c_float,
                                   c_float, c_float, c_float, c_void_p]),
     "lhw_clip_adam": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, c_float, c_float,

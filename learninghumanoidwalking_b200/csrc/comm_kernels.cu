@@ -19,6 +19,12 @@
 // into the CUDA graph of the optimiser step and replayed (every rank replays the same number of steps).  A peer that
 // never arrives does not hang the GPU: the spins are bounded and leave an error word that the host reads with
 // lhw_comm_status once per iteration.  At W = 1 the flag traffic vanishes and this is simply the fused clip + Adam.
+//
+// The adaptive instantiation (<true>, lhw_fused_allreduce_clip_adam_adaptive) adds rsl_rl's KL-adaptive learning rate
+// (DESIGN.md §7.3).  Block 0 of K1 copies this rank's minibatch KL into the KL word of its comm block (after the flag
+// words) before it says "ready"; the last block of K1, after every peer said so and before it says "done reading", sums
+// the W KL words in rank order in float64, divides by W and updates the float64 rate in device memory (same bits on every
+// rank); K2 then takes (float)rate for this very step.  The <false> instantiations are the fixed-rate kernels unchanged.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -36,6 +42,9 @@ namespace {
 constexpr int MAX_WORLD = 16;
 constexpr int COMM_BLOCK = 256;
 constexpr int VEC_PER_THREAD = 1;          // float4 per thread in K1: 154 381 floats -> 151 blocks, one per SM
+constexpr int KL_WORDS = 4;                // after the MAX_WORLD flag words of a comm block: [0] = this rank's KL (float)
+// rsl_rl's adaptive schedule (DESIGN.md §7.3); rl/schedule.py holds the same constants and rule for the host
+constexpr double LR_MIN = 1e-5, LR_MAX = 1e-2, LR_FACTOR = 1.5;
 thread_local std::string g_cerr;
 
 struct Peers {
@@ -70,13 +79,35 @@ __device__ __forceinline__ bool wait_peers(const unsigned int* my_flags, int wor
   return ok;
 }
 
+// the peer's KL word sits right after its MAX_WORLD flag words
+__device__ __forceinline__ float* kl_word(unsigned int* flags) { return reinterpret_cast<float*>(flags + MAX_WORLD); }
+
+// the rule of DESIGN.md §7.3 in IEEE float64; a NaN KL fails every comparison and leaves the rate alone
+__device__ __forceinline__ double adapt_lr(double lr, double kl, double desired_kl) {
+  if (kl > 2.0 * desired_kl) return fmax(LR_MIN, lr / LR_FACTOR);
+  if (kl > 0.0 && kl < desired_kl / 2.0) return fmin(LR_MAX, lr * LR_FACTOR);
+  return lr;
+}
+
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(COMM_BLOCK)
     exchange_reduce_kernel(Peers P, unsigned int* __restrict__ my_flags, unsigned int* __restrict__ state,
                            float* __restrict__ reduced, double* __restrict__ partials, float* __restrict__ coef,
-                           long long n_actor, long long n_total, int rank, int world, float max_norm, long long spin_limit) {
+                           long long n_actor, long long n_total, int rank, int world, float max_norm, long long spin_limit,
+                           const float* __restrict__ kl, double* __restrict__ lr, double desired_kl) {
   __shared__ double sh[2][COMM_BLOCK / 32];
   __shared__ int sh_last;
   const unsigned int epoch = state[ST_EPOCH];
+  if constexpr (ADAPTIVE) {
+    // this rank's KL into its comm block before any "ready": peers read it once they have seen the flag
+    if (blockIdx.x == 0) {
+      if (threadIdx.x == 0) {
+        *kl_word(my_flags) = *kl;
+        __threadfence_system();
+      }
+      __syncthreads();
+    }
+  }
   if (world > 1) {
     // my backward pass precedes this kernel in stream order: the gradient is complete -> tell the peers
     if (blockIdx.x == 0 && (int)threadIdx.x < world) st_release_sys(P.flags[threadIdx.x] + rank, epoch);
@@ -146,15 +177,29 @@ __global__ void __launch_bounds__(COMM_BLOCK)
       state[ST_TICKET] = 0;
     }
   }
+  if constexpr (ADAPTIVE) {
+    // every peer's KL word was written before its "ready", which this block's thread r acquired for peer r
+    __shared__ float sh_kl[MAX_WORLD];
+    if ((int)threadIdx.x < world) sh_kl[threadIdx.x] = __ldcv(kl_word(P.flags[threadIdx.x]));
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double s = 0.0;
+      for (int r = 0; r < world; r++) s += (double)sh_kl[r];     // rank order: the same bits on every rank
+      *lr = adapt_lr(*lr, s / (double)world, desired_kl);
+    }
+  }
   // every block of this rank has consumed the peers' gradients: they may be overwritten
   if (world > 1 && (int)threadIdx.x < world) st_release_sys(P.flags[threadIdx.x] + rank, epoch + 1);
 }
 
-// clip + Adam (rl/algos/ppo.py:393-396) for both networks; coef[0/1] from K1, the Adam step number from device memory
+// clip + Adam (rl/algos/ppo.py:393-396) for both networks; coef[0/1] from K1, the Adam step number from device memory;
+// ADAPTIVE: the rate is (float) of the float64 rate K1 has just updated, the conversion the host applies to a fixed `lr`
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(COMM_BLOCK)
     clip_adam_pair_kernel(const float* __restrict__ reduced, const float* __restrict__ coef, const unsigned int* __restrict__ state,
                           float* __restrict__ param, float* __restrict__ m, float* __restrict__ v, long long n_actor,
-                          long long n_total, float lr, float b1, float b2, float eps) {
+                          long long n_total, float lr, float b1, float b2, float eps, const double* __restrict__ lr_dev) {
+  if constexpr (ADAPTIVE) lr = (float)*lr_dev;
   const float t = (float)(state[ST_STEP] + 1u);
   const float bc1 = 1.0f - powf(b1, t), bc2_sqrt = sqrtf(1.0f - powf(b2, t));
   const float step_size = lr / bc1, coef_a = coef[0], coef_c = coef[1];
@@ -193,6 +238,7 @@ struct lhw_comm {
   double* partials;
   float* coef;           // clip coefficients (actor, critic), then the two gradient norms
   unsigned int* state;   // ST_* words
+  double* lr;            // the adaptive schedule's learning rate (lhw_comm_lr_ptr)
   Peers peers;
   void* opened[MAX_WORLD];
 };
@@ -223,8 +269,8 @@ int lhw_comm_create(lhw_comm** out, long long n_floats, int rank, int world, int
   const char* sl = getenv("LHW_COMM_SPIN_LOG2");
   c->spin_limit = 1ll << (sl && atoi(sl) > 0 && atoi(sl) < 40 ? atoi(sl) : 26);
   const size_t gb = grad_bytes(n_floats);
-  COK(cudaMalloc(&c->block, gb + MAX_WORLD * sizeof(unsigned int)));
-  COK(cudaMemset(c->block, 0, gb + MAX_WORLD * sizeof(unsigned int)));
+  COK(cudaMalloc(&c->block, gb + (MAX_WORLD + KL_WORDS) * sizeof(unsigned int)));
+  COK(cudaMemset(c->block, 0, gb + (MAX_WORLD + KL_WORDS) * sizeof(unsigned int)));
   c->grad = (float*)c->block;
   c->flags = (unsigned int*)(c->block + gb);
   COK(cudaMalloc(&c->reduced, gb));
@@ -241,6 +287,8 @@ int lhw_comm_create(lhw_comm** out, long long n_floats, int rank, int world, int
   COK(cudaMalloc(&c->state, ST_WORDS * sizeof(unsigned int)));
   const unsigned int init[ST_WORDS] = {1u, 0u, 0u, 0u};
   COK(cudaMemcpy(c->state, init, sizeof(init), cudaMemcpyHostToDevice));
+  COK(cudaMalloc(&c->lr, sizeof(double)));
+  COK(cudaMemset(c->lr, 0, sizeof(double)));
   c->peers.grad[rank] = c->grad;
   c->peers.flags[rank] = c->flags;
   *out = c;
@@ -248,6 +296,7 @@ int lhw_comm_create(lhw_comm** out, long long n_floats, int rank, int world, int
 }
 
 void* lhw_comm_grad_ptr(lhw_comm* c) { return c ? c->grad : nullptr; }
+double* lhw_comm_lr_ptr(lhw_comm* c) { return c ? c->lr : nullptr; }
 long long lhw_comm_size(const lhw_comm* c) { return c ? c->n : 0; }
 int lhw_comm_device(const lhw_comm* c) { return c ? c->device : -1; }
 
@@ -286,30 +335,56 @@ int lhw_comm_destroy(lhw_comm* c) {
   cudaFree(c->partials);
   cudaFree(c->coef);
   cudaFree(c->state);
+  cudaFree(c->lr);
   delete c;
   return 0;
 }
 
-int lhw_fused_allreduce_clip_adam(lhw_comm* c, float* param, float* exp_avg, float* exp_avg_sq, long long n_actor,
-                                  long long n_total, float lr, float beta1, float beta2, float eps, float max_norm,
-                                  void* stream) {
+}  // extern "C"
+
+namespace {
+// the three launches of one optimiser step; ADAPTIVE: kl / lr_dev / desired_kl drive the rate (kl, lr_dev unused otherwise)
+template <bool ADAPTIVE>
+int fused_step(lhw_comm* c, float* param, float* exp_avg, float* exp_avg_sq, long long n_actor, long long n_total, float lr,
+               float beta1, float beta2, float eps, float max_norm, const float* kl, double* lr_dev, double desired_kl,
+               void* stream) {
   if (!c || !param || !exp_avg || !exp_avg_sq) return cfail(-1, "null argument");
   if (n_total != c->n || n_actor < 0 || n_actor > n_total) return cfail(-2, "size mismatch");
   cudaStream_t st = (cudaStream_t)stream;
-  exchange_reduce_kernel<<<c->grid, COMM_BLOCK, 0, st>>>(c->peers, c->flags, c->state, c->reduced, c->partials, c->coef, n_actor,
-                                                         n_total, c->rank, c->world, max_norm, c->spin_limit);
+  exchange_reduce_kernel<ADAPTIVE><<<c->grid, COMM_BLOCK, 0, st>>>(c->peers, c->flags, c->state, c->reduced, c->partials, c->coef,
+                                                                   n_actor, n_total, c->rank, c->world, max_norm, c->spin_limit, kl,
+                                                                   lr_dev, desired_kl);
   lhw_count_launch();
   COK(cudaGetLastError());
   int grid2 = (int)((n_total + COMM_BLOCK - 1) / COMM_BLOCK);
   if (grid2 > 132 * 4) grid2 = 132 * 4;   // 4 blocks per SM of an H100 SXM (132 SMs)
-  clip_adam_pair_kernel<<<grid2, COMM_BLOCK, 0, st>>>(c->reduced, c->coef, c->state, param, exp_avg, exp_avg_sq, n_actor, n_total,
-                                                      lr, beta1, beta2, eps);
+  clip_adam_pair_kernel<ADAPTIVE><<<grid2, COMM_BLOCK, 0, st>>>(c->reduced, c->coef, c->state, param, exp_avg, exp_avg_sq, n_actor,
+                                                                n_total, lr, beta1, beta2, eps, lr_dev);
   lhw_count_launch();
   COK(cudaGetLastError());
   exchange_finish_kernel<<<1, 32, 0, st>>>(c->flags, c->state, c->world, c->spin_limit);
   lhw_count_launch();
   COK(cudaGetLastError());
   return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int lhw_fused_allreduce_clip_adam(lhw_comm* c, float* param, float* exp_avg, float* exp_avg_sq, long long n_actor,
+                                  long long n_total, float lr, float beta1, float beta2, float eps, float max_norm,
+                                  void* stream) {
+  return fused_step<false>(c, param, exp_avg, exp_avg_sq, n_actor, n_total, lr, beta1, beta2, eps, max_norm, nullptr, nullptr, 0.0,
+                           stream);
+}
+
+int lhw_fused_allreduce_clip_adam_adaptive(lhw_comm* c, float* param, float* exp_avg, float* exp_avg_sq, long long n_actor,
+                                           long long n_total, const float* kl, double* lr_dev, double desired_kl, float beta1,
+                                           float beta2, float eps, float max_norm, void* stream) {
+  if (!kl || !lr_dev) return cfail(-1, "null argument");
+  if (!(desired_kl > 0.0)) return cfail(-1, "desired_kl must be > 0");
+  return fused_step<true>(c, param, exp_avg, exp_avg_sq, n_actor, n_total, 0.0f, beta1, beta2, eps, max_norm, kl, lr_dev, desired_kl,
+                          stream);
 }
 
 int lhw_comm_status(lhw_comm* c, int* error_word, int* adam_steps, float* norms2, void* stream) {
@@ -332,6 +407,20 @@ int lhw_comm_set_step(lhw_comm* c, int adam_steps, void* stream) {
   if (!c || adam_steps < 0) return cfail(-1, "bad argument");
   const unsigned int v = (unsigned int)adam_steps;
   COK(cudaMemcpyAsync(c->state + ST_STEP, &v, sizeof(v), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  COK(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+
+int lhw_comm_get_lr(lhw_comm* c, double* lr_host, void* stream) {
+  if (!c || !lr_host) return cfail(-1, "null argument");
+  COK(cudaMemcpyAsync(lr_host, c->lr, sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  COK(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+
+int lhw_comm_set_lr(lhw_comm* c, double lr, void* stream) {
+  if (!c || !(lr > 0.0)) return cfail(-1, "bad argument");
+  COK(cudaMemcpyAsync(c->lr, &lr, sizeof(double), cudaMemcpyHostToDevice, (cudaStream_t)stream));
   COK(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
 }

@@ -1,6 +1,6 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
 // torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
-// .fused_exchange.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
+// .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
 // Handles (lhw_sim*, lhw_comm*) travel as int64, as the Python host already holds them.  All ops mutate their output
@@ -274,6 +274,27 @@ void fused_exchange(int64_t comm, Tensor param, Tensor exp_avg, Tensor exp_avg_s
   TORCH_CHECK(rc == 0, "lhw: lhw_fused_allreduce_clip_adam failed (rc=", rc, "): ", lhw_comm_last_error());
 }
 
+void fused_exchange_adaptive(int64_t comm, Tensor param, Tensor exp_avg, Tensor exp_avg_sq, int64_t n_actor, const Tensor& kl, Tensor lr,
+                             double desired_kl, double beta1, double beta2, double eps, double max_norm) {
+  TORCH_CHECK(comm != 0, "lhw: null comm handle");
+  lhw_comm* c = reinterpret_cast<lhw_comm*>(comm);
+  const int64_t n = lhw_comm_size(c);
+  const int dev = lhw_comm_device(c);
+  check_cuda(param, "param", at::kFloat, dev); check_shape(param, "param", {n});
+  check_cuda(exp_avg, "exp_avg", at::kFloat, dev); check_shape(exp_avg, "exp_avg", {n});
+  check_cuda(exp_avg_sq, "exp_avg_sq", at::kFloat, dev); check_shape(exp_avg_sq, "exp_avg_sq", {n});
+  check_cuda(kl, "kl", at::kFloat, dev);
+  TORCH_CHECK(kl.numel() == 1 && kl.dim() <= 1, "lhw: kl has shape ", kl.sizes(), ", expected one float ([] or [1])");
+  check_cuda(lr, "lr", at::kDouble, dev); check_shape(lr, "lr", {1});
+  TORCH_CHECK(n_actor >= 0 && n_actor <= n, "lhw: n_actor out of range");
+  TORCH_CHECK(desired_kl > 0.0, "lhw: desired_kl must be > 0, got ", desired_kl);
+  c10::cuda::CUDAGuard guard(dev);
+  const int rc = lhw_fused_allreduce_clip_adam_adaptive(c, param.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
+                                                        n_actor, n, kl.data_ptr<float>(), lr.data_ptr<double>(), desired_kl, (float)beta1,
+                                                        (float)beta2, (float)eps, (float)max_norm, stream_of(param));
+  TORCH_CHECK(rc == 0, "lhw: lhw_fused_allreduce_clip_adam_adaptive failed (rc=", rc, "): ", lhw_comm_last_error());
+}
+
 }  // namespace
 
 TORCH_LIBRARY(lhw, m) {
@@ -302,6 +323,8 @@ TORCH_LIBRARY(lhw, m) {
         "float beta1, float beta2, float eps, float max_norm, float grad_scale) -> ()");
   m.def("fused_exchange(int comm, Tensor(a!) param, Tensor(b!) exp_avg, Tensor(c!) exp_avg_sq, int n_actor, float lr, float beta1, float beta2, "
         "float eps, float max_norm) -> ()");
+  m.def("fused_exchange_adaptive(int comm, Tensor(a!) param, Tensor(b!) exp_avg, Tensor(c!) exp_avg_sq, int n_actor, Tensor kl, "
+        "Tensor(d!) lr, float desired_kl, float beta1, float beta2, float eps, float max_norm) -> ()");
 }
 
 // CompositeExplicitAutograd: the checks must also reject CPU tensors with OUR message (a CUDA-only registration would answer
@@ -321,4 +344,5 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("grad_sumsq", &grad_sumsq);
   m.impl("clip_adam_dev", &clip_adam_dev);
   m.impl("fused_exchange", &fused_exchange);
+  m.impl("fused_exchange_adaptive", &fused_exchange_adaptive);
 }

@@ -54,6 +54,36 @@ class PeerComm:
         (the Adam step number and the barrier epoch live in device memory)."""
         _lib.ops().fused_exchange(self._h.value, param, exp_avg, exp_avg_sq, int(n_actor), lr, betas[0], betas[1], eps, max_norm)
 
+    def fused_step_adaptive(self, param, exp_avg, exp_avg_sq, n_actor, kl, desired_kl, betas, eps, max_norm):
+        """fused_step with the KL-adaptive rate (DESIGN.md §7.3): kl is this rank's minibatch KL (one float32 device scalar); the
+        rate is self.lr, in device memory, updated from the ranks' mean KL before this step's Adam update uses it."""
+        _lib.ops().fused_exchange_adaptive(self._h.value, param, exp_avg, exp_avg_sq, int(n_actor), kl, self.lr, float(desired_kl),
+                                           betas[0], betas[1], eps, max_norm)
+
+    @property
+    def lr(self) -> torch.Tensor:
+        """The adaptive schedule's float64 rate word of this comm, as a [1] device tensor."""
+        if getattr(self, "_lr", None) is None:
+            L = _lib.lib()
+            ptr = L.lhw_comm_lr_ptr(self._h)
+            arr = _CudaArray(ptr, 1)
+            arr.__cuda_array_interface__["typestr"] = "<f8"
+            self._lr_keep = arr
+            self._lr = torch.as_tensor(arr, device=self.grad.device)
+            assert self._lr.data_ptr() == ptr
+        return self._lr
+
+    def get_lr(self) -> float:
+        """The device rate (synchronises the current stream)."""
+        v = ctypes.c_double(0.0)
+        if _lib.lib().lhw_comm_get_lr(self._h, ctypes.byref(v), _lib.current_stream_ptr()):
+            raise _lib.LhwError(f"lhw_comm_get_lr failed: {_lib.lib().lhw_comm_last_error().decode()}")
+        return v.value
+
+    def set_lr(self, lr: float):
+        if _lib.lib().lhw_comm_set_lr(self._h, float(lr), _lib.current_stream_ptr()):
+            raise _lib.LhwError(f"lhw_comm_set_lr failed: {_lib.lib().lhw_comm_last_error().decode()}")
+
     def status(self):
         """(completed Adam steps, (actor grad norm, critic grad norm) of the last step); raises if a peer did not arrive at the
         gradient exchange within the spin limit (the kernels carry on with partial sums rather than hang the GPU).
@@ -71,5 +101,6 @@ class PeerComm:
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
+            self._lr = None
             _lib.lib().lhw_comm_destroy(self._h)
             self._h = ctypes.c_void_p()

@@ -24,7 +24,7 @@ from torch.nn import functional as F
 
 from .. import _lib
 from .optim import FusedClipAdam
-from . import snapshot
+from . import schedule, snapshot
 from .policies import FF_V, Gaussian_FF_Actor
 from .snapshot import SnapshotError, plain_args
 from .storage import BatchData
@@ -73,6 +73,9 @@ class PPO:
         self.eval_batches = getattr(args, "eval_batches", 5)     # evaluate(num_batches=5) in the reference
         self.eval_at_start = getattr(args, "eval_at_start", True)  # the reference evaluates (and checkpoints) at iteration 0
         self.imitate_coeff = getattr(args, "imitate_coeff", 0.0)
+        # `--schedule adaptive`: the KL-adaptive rate of DESIGN.md §7.3, held in device memory by the fused exchange
+        self.schedule, self.desired_kl = schedule.schedule_of(args)
+        schedule.check(self.schedule, self.desired_kl)
         # opt-in: TF32 tensor-core GEMMs for the MLPs (the reference trains in fp32 with torch's default allow_tf32 = False, and
         # so does this build unless asked otherwise; at minibatches >= 32k the update is GEMM bound)
         if getattr(args, "tf32", False):
@@ -185,7 +188,14 @@ class PPO:
                     step_count=[a_opt.step_count, c_opt.step_count], adam_step_dev=dev,
                     obs_norm={f"{net}.{name}": cpu(getattr(getattr(self, net), name))
                               for net in ("policy", "critic") for name in ("obs_mean", "obs_std")},
-                    best_eval=float(self._best_eval), total_steps=int(self.total_steps), elapsed=float(elapsed))
+                    best_eval=float(self._best_eval), total_steps=int(self.total_steps), elapsed=float(elapsed),
+                    **self._schedule_state())
+
+    def _schedule_state(self) -> dict:
+        """The adaptive schedule's device rate (its float64 bits) for a snapshot; nothing under the fixed schedule."""
+        if getattr(self, "schedule", "fixed") != "adaptive":
+            return {}
+        return dict(adaptive_lr=torch.tensor([self._comm.get_lr()], dtype=torch.float64))
 
     def snapshot_shard(self, itr: int) -> dict:
         """This rank's part of the snapshot: its environments' records and its sampler's state."""
@@ -227,6 +237,10 @@ class PPO:
             env.state_i.copy_(shard["state_i"])
         env._fresh = bool(shard["fresh"])
         a_opt.step_count, c_opt.step_count = learner["step_count"]
+        if getattr(self, "schedule", "fixed") == "adaptive":
+            if "adaptive_lr" not in learner:
+                raise SnapshotError("the snapshot holds no learning rate of the adaptive schedule (was it written by a fixed-rate run?)")
+            self._comm.set_lr(float(learner["adaptive_lr"][0]))
         if self._comm is not None:
             self._comm.set_step(learner["adam_step_dev"][0])
         else:
@@ -342,8 +356,16 @@ class PPO:
             a_opt.step_count += 1
             c_opt.step_count += 1
             g = a_opt.param_groups[0]
-            self._comm.fused_step(self._flat_param, self._flat_m, self._flat_v, self._n_actor, g["lr"], g["betas"], g["eps"],
-                                  g["max_norm"])
+            if getattr(self, "schedule", "fixed") == "adaptive":
+                # scalar 3, the minibatch's "Mean KL Div", drives the device rate; the same launches eager and in the graph
+                self._comm.fused_step_adaptive(self._flat_param, self._flat_m, self._flat_v, self._n_actor,
+                                               scalars[3].detach().float().reshape(1), self.desired_kl, g["betas"], g["eps"],
+                                               g["max_norm"])
+            else:
+                self._comm.fused_step(self._flat_param, self._flat_m, self._flat_v, self._n_actor, g["lr"], g["betas"], g["eps"],
+                                      g["max_norm"])
+        elif getattr(self, "schedule", "fixed") == "adaptive":
+            self._check_schedule()
         elif isinstance(a_opt, FusedClipAdam) and isinstance(c_opt, FusedClipAdam):
             if self.world > 1:  # baseline path: NCCL all-reduce of the flat gradient, then clip+Adam launches
                 dist.all_reduce(self._flat_grad, op=dist.ReduceOp.SUM)
@@ -425,6 +447,9 @@ class PPO:
         self.critic_optimizer = FusedClipAdam(self.critic, lr=self.lr, eps=self.eps, max_norm=self.grad_clip,
                                               views=(sl(flat, 1), sl(grad, 1), sl(self._flat_m, 1), sl(self._flat_v, 1)))
         self.actor_optimizer.world = self.critic_optimizer.world = self.world
+        if getattr(self, "schedule", "fixed") == "adaptive":
+            self._check_schedule()
+            self._comm.set_lr(self.lr)      # `--lr` is the starting rate (so also after `--continued`)
         if self.world > 1:
             # replicas start from rank 0's weights whatever the seeding of the ranks was
             dist.broadcast(self._flat_param, src=0)
@@ -435,6 +460,17 @@ class PPO:
         for w in self.workers:
             w.invalidate_graphs()
         self._ug, self._ug_calls = None, 0
+
+    def _check_schedule(self):
+        """The adaptive schedule lives on the fused exchange only: refuse the baseline exchange and hand-assigned optimisers."""
+        if getattr(self, "schedule", "fixed") != "adaptive":
+            return
+        if not (isinstance(self.actor_optimizer, FusedClipAdam) and isinstance(self.critic_optimizer, FusedClipAdam)):
+            raise ValueError("--schedule adaptive drives the fused exchange's device rate; hand-assigned torch optimisers "
+                             "would ignore it (use make_optimizers())")
+        if self._comm is None:
+            raise ValueError("--schedule adaptive needs the fused exchange, which holds the rate in device memory; "
+                             "LHW_FUSED_EXCHANGE=0 selects the baseline exchange, which has no adaptive schedule")
 
     # ------------------------------------------------------------------ device data path helpers
     def normalize_advantages(self, returns: torch.Tensor, values: torch.Tensor, from_rollout: bool = False) -> torch.Tensor:
@@ -511,6 +547,7 @@ class PPO:
         elapsed time and fps carry on, and the TensorBoard scalars the stopped run logged from start_itr on are dropped."""
         if self.actor_optimizer is None:
             self.make_optimizers()
+        self._check_schedule()
         env = self.env
         obs_mirr = getattr(env, "mirror_clock_observation", None) if self.mirror_coeff else None
         act_mirr = getattr(env, "mirror_action", None) if self.mirror_coeff else None
@@ -549,6 +586,8 @@ class PPO:
             stats = (stats / max(1, n_updates)).tolist()   # the only host sync of the optimisation phase
             if getattr(self, "_comm", None) is not None:
                 self._comm.status()    # raises if a peer missed a gradient exchange (bounded spin in the kernels)
+            adaptive = getattr(self, "schedule", "fixed") == "adaptive"
+            lr_now = self._comm.get_lr() if adaptive else None     # the stream has just been synchronised
             optimize_time = time.time() - t1
             total_time = time.time() - train_start
             fps = self.total_steps / total_time
@@ -557,13 +596,16 @@ class PPO:
             log.append(dict(itr=itr, sample_time=sample_time, optimize_time=optimize_time, fps=fps, ep_rew=ep_rew, ep_len=ep_len,
                             actor_loss=stats[0], entropy=stats[1], critic_loss=stats[2], kl=stats[3], mirror=stats[4],
                             clip_frac=stats[6]))
+            if adaptive:
+                log[-1]["lr"] = lr_now
             if verbose and self.rank == 0:
                 print(f"Optimizer took: {optimize_time:.2f}s")
                 print("-" * 37)
                 for k, v in (("Mean Eprew", ep_rew), ("Mean Eplen", ep_len), ("Actor loss", stats[0]), ("Critic loss", stats[2]),
                              ("Mirror loss", stats[4]), ("Imitation loss", stats[5]), ("Mean KL Div", stats[3]),
                              ("Mean Entropy", stats[1]), ("Clip Fraction", stats[6]),
-                             ("Mean noise std", float(torch.as_tensor(self.policy.stds).mean()))):
+                             ("Mean noise std", float(torch.as_tensor(self.policy.stds).mean())),
+                             *((("Learning rate", lr_now),) if adaptive else ())):
                     print(f"| {k:>15} | {v:>15.5g} |")
                 print("-" * 37)
                 eta = round((n_itr - itr) * total_time / (itr + 1))
@@ -574,7 +616,7 @@ class PPO:
                                ("Loss/imitation", stats[5]), ("Train/mean_reward", ep_rew), ("Train/mean_episode_length", ep_len),
                                ("Train/mean_noise_std", float(torch.as_tensor(self.policy.stds).mean())), ("Time/fps", fps),
                                ("Time/sample_time", sample_time), ("Time/optimize_time", optimize_time),
-                               ("Time/total_elapsed", total_time)):
+                               ("Time/total_elapsed", total_time), *((("Train/learning_rate", lr_now),) if adaptive else ())):
                     writer.add_scalar(tag, v, itr)
             if (itr == 0 and getattr(self, "eval_at_start", True)) or (itr + 1) % self.eval_freq == 0:     # rl/algos/ppo.py:597-615
                 t2 = time.time()

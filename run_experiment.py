@@ -14,7 +14,8 @@ control step, ray-cast on the GPU (BatchedHumanoidEnv.render_rgb: inertia boxes,
 the reference's meshes) and encoded with OpenCV, where the reference's EvaluateEnv uses MuJoCo's offscreen renderer.
 Artefacts keep the reference's names and format: `<logdir>/<timestamp>_<env>/experiment.pkl`, `actor_<itr>.pt`,
 `critic_<itr>.pt` (whole pickled modules, rl/utils/checkpointer.py:51-83); `train --imitate PATH` also keeps a copy of the
-teacher as `teacher.pt` (DESIGN §7.2).
+teacher as `teacher.pt` (DESIGN §7.2).  `train --schedule adaptive [--desired-kl 0.01]` adapts the learning rate to the policy's
+KL after every minibatch (rsl_rl's schedule, DESIGN §7.3); the rate is printed and logged as `Train/learning_rate`.
 """
 import argparse
 import os
@@ -54,6 +55,9 @@ TRAIN_FLAGS = [
                                help="auto: --minibatch-size is scaled by (this rank's batch / 4800) so that an iteration keeps the reference's "
                                     "225 optimiser steps at its default flags; off: --minibatch-size samples per rank, literally")),
     ("--snapshot", dict(action="store_true", help="at every checkpoint, also snapshot the whole training state for `resume`")),
+    ("--schedule", dict(type=_S, default="fixed", choices=["fixed", "adaptive"],
+                        help="learning rate: fixed at --lr, or adaptive: starts at --lr and follows the minibatch KL (DESIGN §7.3)")),
+    ("--desired-kl", dict(type=_F, default=0.01, help="target KL of --schedule adaptive")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -142,6 +146,19 @@ def make_env_fn(args, rank, world, local):
     return env_fn
 
 
+def check_schedule(args):
+    """Refuse a learning-rate schedule this launch cannot run, before any environment or run directory exists."""
+    from learninghumanoidwalking_b200.rl import schedule
+    kind, desired_kl = schedule.schedule_of(args)
+    try:
+        schedule.check(kind, desired_kl)
+    except ValueError as e:
+        raise SystemExit(f"train --schedule {kind}: {e}")
+    if kind == "adaptive" and os.environ.get("LHW_FUSED_EXCHANGE", "1") == "0":
+        raise SystemExit("train --schedule adaptive: the rate lives on the fused exchange, and LHW_FUSED_EXCHANGE=0 selects the "
+                         "baseline exchange, which has no adaptive schedule")
+
+
 def run_experiment(args):
     from learninghumanoidwalking_b200.rl import PPO
     rank, world, local = _dist_setup()
@@ -157,6 +174,7 @@ def run_experiment(args):
         print_system_info(args)
     if args.recurrent:
         raise NotImplementedError("--recurrent is outside the accelerated path (SURVEY.md §2)")
+    check_schedule(args)
     if args.imitate:
         # the teacher, its env and the projector to this env are checked before any environment or run directory exists
         from learninghumanoidwalking_b200.rl import imitation
@@ -208,6 +226,7 @@ def resume(args):
         if rank == 0:
             print(f"Nothing to do: the snapshot of {run_dir} is at iteration {start - 1} of {n_itr}.")
         return None
+    check_schedule(run_args)      # an experiment.pkl without a schedule is a fixed-rate run
     rank, world, local = _dist_setup()
     run_args.logdir, run_args.n_itr, run_args.snapshot = run_dir, n_itr, True
     if run_args.yaml is not None and Path(run_dir, Path(run_args.yaml).name).exists():

@@ -30,6 +30,11 @@ Imitation (opt-in, `--imitation`, IMITATION_CASES): the CUDA learner trains with
 and S carries a float64 copy of the same teacher behind the same projector, so that its non-fused branch computes the
 reference's term (rl/algos/ppo.py:361-368).  Without a teacher S is the shadow above, unchanged.
 
+Adaptive learning rate (opt-in, `--adaptive`, ADAPTIVE_CASES): the CUDA learner runs `--schedule adaptive` (DESIGN §7.3).  The
+old policy is re-offset before every step, alternately far and near, so that the minibatch KL crosses both thresholds of a
+desired_kl chosen from a probe.  After each step the device rate must equal the float64 rule (rl/schedule.py) applied to the
+CUDA learner's own KL, bit for bit, and both shadows step with that rate.
+
 `python tools/learner_local_error.py` prints the distribution tables (needs a GPU); `--rehearse` runs the float64 parts on the
 CPU at a tiny size.
 """
@@ -240,20 +245,30 @@ def _rel(d, ref):
 
 def compare_step(ppo, sh, sh_opt, ob, ab, rb, db, obs_mirr, act_mirr):
     """One re-synchronised optimiser step of the CUDA learner `ppo` and of the shadows; returns the errors of this step, each
-    divided by its bound (<= 1 passes), plus diagnostics."""
+    divided by its bound (<= 1 passes), plus diagnostics.  Under the adaptive schedule the shadows take the rate the device
+    computed for this step, and the record holds it (lr0 -> lr1) with the rule's value for the learner's KL (lr_rule)."""
+    from learninghumanoidwalking_b200.rl.schedule import adapt_lr
+    adaptive = getattr(ppo, "schedule", "fixed") == "adaptive"
     flat0, m0, v0 = ppo._flat_param.clone(), ppo._flat_m.clone(), ppo._flat_v.clone()
     step0 = adam_steps(ppo)
     assert ppo.actor_optimizer.step_count == ppo.critic_optimizer.step_count == step0
     sh.load(flat0, m0, v0, step0, ppo.old_policy)
     near = int(sh.near_kink(ob, ab).sum())
+    lr0 = ppo._comm.get_lr() if adaptive else ppo.lr
     out = ppo._update_step(ob, ab, rb, db, obs_mirr, act_mirr).double().cpu()
     torch.cuda.synchronize()
     assert adam_steps(ppo) == step0 + 1
+    lr = ppo._comm.get_lr() if adaptive else ppo.lr
+    for s in (sh, sh_opt):
+        for opt in (s.ppo.actor_optimizer, s.ppo.critic_optimizer):
+            opt.param_groups[0]["lr"] = lr
     g_cuda, n_cuda = cuda_grads(ppo), preclip_norms(ppo)
     ref, g_ref, n_ref = sh.step(ob, ab, rb, db)
     sh_opt.load(flat0, m0, v0, step0)
     sh_opt.optimise(g_cuda)
     e = dict(near=near, norms=n_cuda, norms_ref=n_ref, clipped=tuple(n > ppo.grad_clip for n in n_cuda), scalars=out.tolist())
+    if adaptive:     # out[3] is the learner's float32 KL, widened exactly
+        e.update(lr0=lr0, lr1=lr, kl=float(out[3]), kl_ref=ref[3], lr_rule=adapt_lr(lr0, float(out[3]), ppo.desired_kl))
     e["scalar"] = max(abs(float(out[k]) - ref[k]) / max(1.0, abs(ref[k])) for k in range(7)) / BOUNDS["scalar"]
     g_ref = [g.reshape(-1) for g in g_ref]
     l2 = [_rel((a.double() - b).norm(), b.norm()) for a, b in zip(g_cuda, g_ref)]
@@ -271,9 +286,9 @@ def compare_step(ppo, sh, sh_opt, ob, ab, rb, db, obs_mirr, act_mirr):
     e["moment"] = mom[sh_opt] / BOUNDS["moment"]
     e["moment_vs_shadow"] = mom[sh]
     p_new, p_opt, p_ref = ppo._flat_param.double().to(sh.device), sh_opt.flat("param"), sh.flat("param")
-    allowed = ulp32(p_opt) + PARAM_LR * ppo.lr
+    allowed = ulp32(p_opt) + PARAM_LR * lr
     e["param"] = float(((p_new - p_opt).abs() / allowed).max()) / BOUNDS["param"]
-    e["param_vs_shadow_lr"] = float((p_new - p_ref).abs().max()) / ppo.lr      # reported: S's own step, not bounded
+    e["param_vs_shadow_lr"] = float((p_new - p_ref).abs().max()) / lr      # reported: S's own step, not bounded
     return e
 
 
@@ -284,6 +299,23 @@ def offset_mean_(policy, seed, scale=0.01):
     with torch.no_grad():
         b = policy.means.bias
         b.add_((scale * torch.randn(b.shape, generator=g, dtype=torch.float64)).to(b.device, b.dtype))
+
+
+def reoffset_(old, policy, seed, scale):
+    """old = policy with its mean output offset by N(0, scale^2) per action, in place (a captured graph keeps its addresses)."""
+    with torch.no_grad():
+        for q, p in zip(old.parameters(), policy.parameters()):
+            q.copy_(p)
+    offset_mean_(old, seed, scale)
+
+
+def choose_desired_kl(kls, far):
+    """desired_kl that puts every probed step with far[k] above 2 desired_kl and every other below desired_kl / 2, at the
+    geometric middle of the gap."""
+    hi = min(k for k, f in zip(kls, far) if f)
+    lo = max(k for k, f in zip(kls, far) if not f)
+    assert hi > 8 * lo > 0, f"the probed KLs do not straddle a factor-4 band with margin: {kls}"
+    return float(np.sqrt(hi * lo))
 
 
 def choose_max_norm(norms, regime):
@@ -323,10 +355,12 @@ def teacher_file(env):
 
 
 def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, steps=7, regime="critic", learn_std=False,
-                  mirror=True, seed=0, hyper=None, imitate=None, imitate_coeff=2.0):
+                  mirror=True, seed=0, hyper=None, imitate=None, imitate_coeff=2.0, kl_scales=None):
     """Build the CUDA learner on a sampled batch of `model`, choose max_grad_norm for `regime`, run `steps` re-synchronised steps
     through _update_step (3 eager warm-ups, then the captured graph).  LHW_* switches come from the caller's environment.
     imitate: the env of a teacher (teacher_file) to train with, at imitate_coeff; the shadows then carry its float64 copy.
+    kl_scales: the adaptive schedule: before step k the old policy is the policy offset by kl_scales[k] (reoffset_), and
+    desired_kl is chosen from a probe so that the far steps (the larger scale) decrease the rate and the others increase it.
     Returns (list of per-step error dicts, max_grad_norm)."""
     from learninghumanoidwalking_b200.envs import BatchedHumanoidEnv
     from learninghumanoidwalking_b200.rl import PPO
@@ -346,6 +380,9 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
                            steps_per_env=steps_per_env, eval_batches=0, eval_at_start=False, logdir="/tmp/lhw_learner_local_error")
     if imitate is not None:
         args.imitate, args.imitate_coeff = teacher_file(imitate), imitate_coeff
+    if kl_scales is not None:
+        assert len(kl_scales) == steps
+        args.schedule, args.desired_kl = "adaptive", 0.01     # desired_kl is chosen below
     ppo = PPO(env_fn, args, seed=seed)
     teach = dict(teacher=ppo.base_policy, projector=ppo.imitation_projector, imitate_coeff=ppo.imitate_coeff) \
         if imitate is not None else {}
@@ -365,8 +402,17 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
         i = cand[~sh.near_kink(obs[cand], act[cand])][:B]
         assert i.numel() == B, f"only {i.numel()} of {C} candidates are away from the loss's kinks"
         return i
-    norms = [probe.step(obs[i], act[i], ret[i], adv[i] * s)[2] for i, s in ((first(c, probe), s) for c, s in zip(perm, scale))]
+    norms, kls = [], []
+    for k, (c, s) in enumerate(zip(perm, scale)):
+        if kl_scales is not None:
+            reoffset_(probe.old_policy, probe.policy, seed + k, kl_scales[k])
+        i = first(c, probe)
+        out, _, n = probe.step(obs[i], act[i], ret[i], adv[i] * s)
+        norms.append(n)
+        kls.append(out[3])
     ppo.grad_clip = choose_max_norm(norms, regime)
+    if kl_scales is not None:
+        ppo.desired_kl = choose_desired_kl(kls, [x == max(kl_scales) for x in kl_scales])
     ppo.make_optimizers()
     offset_mean_(ppo.old_policy, seed)
     sh = Shadow(ppo.policy, ppo.old_policy, ppo.critic, hyper_of(ppo), sym, device=ppo.device, **teach)
@@ -374,7 +420,9 @@ def per_step_case(model="jvrc_walk", B=21845, n_envs=4096, steps_per_env=44, ste
     obs_mirr = getattr(ppo.env, "mirror_clock_observation", None) if mirror else None
     act_mirr = getattr(ppo.env, "mirror_action", None) if mirror else None
     res = []
-    for cand, s in zip(perm, scale):
+    for k, (cand, s) in enumerate(zip(perm, scale)):
+        if kl_scales is not None:
+            reoffset_(ppo.old_policy, ppo.policy, seed + k, kl_scales[k])
         # the minibatch skips the samples at a kink of the loss (Shadow.near_kink): there the two precisions may legitimately
         # take different branches, and one such sample moves a gradient far more than rounding does
         sh.load(ppo._flat_param, ppo._flat_m, ppo._flat_v, adam_steps(ppo), ppo.old_policy)
@@ -552,6 +600,15 @@ IMITATION_CASES = {
 }
 
 
+# opt-in (--adaptive): `--schedule adaptive`; the old policy alternates far / near, so the rate goes down and up again
+ADAPTIVE_CASES = {
+    "adaptive_jvrc_walk_B21845": (dict(model="jvrc_walk", B=21845, regime="both",
+                                       kl_scales=[0.03, 0.003, 0.03, 0.003, 0.003, 0.03, 0.003]), {}),
+    "adaptive_learn_std_B4097": (dict(model="jvrc_walk", B=4097, regime="both", learn_std=True, n_envs=1024, steps_per_env=32,
+                                      kl_scales=[0.03, 0.003, 0.03, 0.003, 0.003, 0.03, 0.003]), {}),
+}
+
+
 @contextlib.contextmanager
 def switches(env):
     old = {k: os.environ.get(k) for k in env}
@@ -599,15 +656,17 @@ def main():
     ap.add_argument("--cases", default=",".join(CASES))
     ap.add_argument("--iterations", default="jvrc_walk,h1", help="whole-iteration tier variants ('' skips it)")
     ap.add_argument("--imitation", action="store_true", help="also the per-step cases with a teacher (IMITATION_CASES)")
+    ap.add_argument("--adaptive", action="store_true", help="also the per-step cases of the adaptive schedule (ADAPTIVE_CASES)")
     args = ap.parse_args()
     if args.rehearse:
         print(rehearse())
         return
     print("| case | quantity | median | p99 | max | bound |\n|---|---|---|---|---|---|")
     notes = []
-    names = [c for c in args.cases.split(",") if c] + (list(IMITATION_CASES) if args.imitation else [])
+    names = [c for c in args.cases.split(",") if c] + (list(IMITATION_CASES) if args.imitation else []) \
+        + (list(ADAPTIVE_CASES) if args.adaptive else [])
     for name in names:
-        kw, env = {**CASES, **IMITATION_CASES}[name]
+        kw, env = {**CASES, **IMITATION_CASES, **ADAPTIVE_CASES}[name]
         t0 = time.time()
         with switches(env):
             res, mn = per_step_case(**kw)
@@ -617,7 +676,8 @@ def main():
                      f"near {[e['near'] for e in res]}, graph {[e['graph'] for e in res]}, "
                      f"param vs S / lr {max(e['param_vs_shadow_lr'] for e in res):.2e}, "
                      f"moments vs S {max(e['moment_vs_shadow'] for e in res):.1e}, "
-                     f"grad l2 per tensor {[e['grad_l2_per_tensor'] for e in res]}")
+                     f"grad l2 per tensor {[e['grad_l2_per_tensor'] for e in res]}"
+                     + (", kl " + str([round(e["kl"], 6) for e in res]) + ", lr " + str([e["lr1"] for e in res]) if "lr1" in res[0] else ""))
     print("\n".join(notes), flush=True)
     for name in [c for c in args.iterations.split(",") if c]:
         kw = dict(model="jvrc_walk") if name == "jvrc_walk" else dict(model="h1", n_envs=1024, steps=100)
