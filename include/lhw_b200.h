@@ -90,6 +90,18 @@ int lhw_sim_render(lhw_sim* sim, const void* state_r, const int32_t* state_i, in
                    int width, int height, double dx, double dy, double z, double distance, double azimuth, double elevation,
                    double fovy, uint8_t* rgb, void* stream);
 
+/* lhw_sim_eval_accumulate: evaluation statistics of one control step, on the device (DESIGN.md §7.4; the reference only has
+ * EvaluateEnv's single roll-out, rl/utils/eval.py).  After an lhw_sim_step with autoreset == 0 it reads the step's reward [n],
+ * rew_terms [n,10] and done [n] and the records state_r / state_i (only read) and updates acc [n, lhw_sim_eval_words()]
+ * float64 (zero it before the first step).  Per env, while its ended-by-done word is 0: episode length, return, ended-by-done
+ * (set by the step whose done is set, which is counted), the 10 reward-term sums; walking tasks (and h1 against zero
+ * references), per mode STANDING / INPLACE / FORWARD: steps and the sums of |v_fwd - vx_ref|, |v_lat - vy_ref|, |w_z - yaw_ref|
+ * with the references zeroed as the reward zeroes them; jvrc_step: footstep targets reached and sequence length.  The word
+ * layout is sim_core.h's EV_* enum. */
+int lhw_sim_eval_words(void);
+int lhw_sim_eval_accumulate(lhw_sim* sim, const void* state_r, const int32_t* state_i, int n_envs, const void* reward,
+                            const void* rew_terms, const int32_t* done, double* acc, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

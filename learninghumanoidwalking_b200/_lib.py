@@ -32,6 +32,8 @@ SIGNATURES = {
     "lhw_sim_set_step_height": (c_int, [c_void_p, ctypes.c_double]),
     "lhw_sim_render": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int] + [ctypes.c_double] * 7
                        + [c_void_p, c_void_p]),
+    "lhw_sim_eval_words": (c_int, []),
+    "lhw_sim_eval_accumulate": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 5),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

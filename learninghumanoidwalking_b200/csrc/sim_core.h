@@ -2348,4 +2348,59 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
   LHW_SYNC();
 }
 
+// ================================================================= evaluation statistics (lhw_sim_eval_accumulate, DESIGN.md §7.4)
+// Per env, float64 words: episode length, return, ended-by-done flag, the NREW reward-term sums; per walking mode m
+// (STANDING / INPLACE / FORWARD) at EV_TRACK + 4 m: steps in m and the sums of |v_fwd - vx_ref|, |v_lat - vy_ref|,
+// |w_z - yaw_ref|; the SteppingTask's target index t1 (= footsteps reached) and sequence length at the last counted step.
+// Words a variant has no use for stay 0.
+enum { EV_LEN = 0, EV_RET = 1, EV_DONE = 2, EV_TERMS = 3, EV_TRACK = EV_TERMS + NREW, EV_REACHED = EV_TRACK + 12, EV_SEQLEN,
+       EV_WORDS };
+
+// The positions eval_accumulate_env reads in the state record: the persistent block of Work, which load_state / store_state
+// copy in the order Persist [+ PersistStep] declares it, and the int record's mode word (load_state: w.mode = si[1]).
+template <class real, int NJ, int TK> struct RecordAt {
+  static constexpr int NV = 6 + 2 * NJ, NQ = NV + 1, NU = 2 * NJ;
+  static constexpr int QPOS = 0, QVEL = NQ, MODE_REF = NQ + 2 * NV + 5 * NU, TK_WORDS = MODE_REF + 4 + 4 * NSLAB;
+  static constexpr int I_MODE = 1;
+  static_assert(sizeof(Persist<real, NJ, TK>) == sizeof(real) * (MODE_REF + 4) &&
+                    sizeof(PersistStep<real, NJ, TK>) == sizeof(real) * (TK_WORDS + 5),
+                "RecordAt must follow the persistent block of Work");
+};
+
+// One control step of one env into its accumulator acc[EV_WORDS], from the step's outputs (reward, rew_terms[NREW], done) and
+// the record it left (autoreset off).  An env counts the steps up to and including the first with done set; after that its
+// EV_DONE word is 1 and it adds nothing.  The walking-task references are zeroed as the reward zeroes them; v is the
+// record's qvel[0:3] in the root frame of qpos[3:7] and w_z is qvel[5] (the reward's root velocity lags these by one substep).
+template <class real, int NJ, int TK>
+LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward, const real* rew_terms, int32_t done, double* acc) {
+  using A = RecordAt<real, NJ, TK>;
+  if (acc[EV_DONE] != 0) return;
+  acc[EV_LEN] += 1;
+  acc[EV_RET] += (double)reward;
+  for (int k = 0; k < NREW; k++) acc[EV_TERMS + k] += (double)rew_terms[k];
+  if constexpr (Cfg<NJ, TK>::STEP) {
+    acc[EV_REACHED] = (double)sr[A::TK_WORDS + 1];
+    acc[EV_SEQLEN] = (double)sr[A::TK_WORDS + 0];
+  } else {
+    const int mode = Cfg<NJ, TK>::STAND ? (int)STANDING : si[A::I_MODE];   // the StandingTask holds zero references
+    double yaw_ref = (double)sr[A::MODE_REF + 0], vx = (double)sr[A::MODE_REF + 1], vy = (double)sr[A::MODE_REF + 2];
+    if (mode == STANDING) { yaw_ref = vx = vy = 0; }
+    else if (mode == INPLACE) { vx = vy = 0; }
+    else { yaw_ref = 0; }
+    const double qw = (double)sr[A::QPOS + 3], x = (double)sr[A::QPOS + 4], y = (double)sr[A::QPOS + 5], z = (double)sr[A::QPOS + 6];
+    const double s = 2 / (qw * qw + x * x + y * y + z * z);
+    const double X = x * s, Y = y * s, Z = z * s;
+    const double wX = qw * X, wY = qw * Y, wZ = qw * Z, xX = x * X, xY = x * Y, xZ = x * Z, yY = y * Y, yZ = y * Z, zZ = z * Z;
+    const double v0 = (double)sr[A::QVEL + 0], v1 = (double)sr[A::QVEL + 1], v2 = (double)sr[A::QVEL + 2];
+    const double vf = (1 - (yY + zZ)) * v0 + (xY + wZ) * v1 + (xZ - wY) * v2;   // (R^T v)[0]
+    const double vl = (xY - wZ) * v0 + (1 - (xX + zZ)) * v1 + (yZ + wX) * v2;   // (R^T v)[1]
+    double* t = acc + EV_TRACK + 4 * mode;
+    t[0] += 1;
+    t[1] += m_abs(vf - vx);
+    t[2] += m_abs(vl - vy);
+    t[3] += m_abs((double)sr[A::QVEL + 5] - yaw_ref);
+  }
+  if (done) acc[EV_DONE] = 1;
+}
+
 }  // namespace lhw

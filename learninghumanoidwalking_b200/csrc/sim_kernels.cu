@@ -172,6 +172,19 @@ __global__ void __launch_bounds__(sizeof(real) == 8 ? LHW_X_REGCAP : 896, 1)
   if (alive) store_state<real, NJ, TK>(w, sr, si);
 }
 
+// evaluation statistics: one thread per env (a few dozen words read and written per env, no cross-env work; the record is read
+// in place, nothing of it is written)
+template <class real, int NJ, int TK>
+__global__ void __launch_bounds__(256) eval_accumulate_kernel(const real* __restrict__ state_r, const int32_t* __restrict__ state_i,
+                                                             int n_envs, const real* __restrict__ reward,
+                                                             const real* __restrict__ rew_terms, const int32_t* __restrict__ done,
+                                                             double* __restrict__ acc) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= n_envs) return;
+  eval_accumulate_env<real, NJ, TK>(state_r + (size_t)env * Dims<real, NJ, TK>::NSTATE_R, state_i + (size_t)env * NSTATE_I, reward[env],
+                                    rew_terms + (size_t)env * NREW, done[env], acc + (size_t)env * EV_WORDS);
+}
+
 }  // namespace
 
 // what every sim has, whichever its variant; SimOf<real, NJ, TK> holds its model and launches its kernels
@@ -188,6 +201,8 @@ struct lhw_sim {
                     int32_t* ended, int32_t* ep_len, void* ep_rew, cudaStream_t st) = 0;
   virtual void render(const void* state_r, const int32_t* state_i, int n_envs, const int32_t* env_ids, int n_ids, int width,
                       int height, const render::Camera& cam, uint8_t* rgb, cudaStream_t st) = 0;
+  virtual void eval_accumulate(const void* state_r, const int32_t* state_i, int n_envs, const void* reward, const void* rew_terms,
+                               const int32_t* done, double* acc, cudaStream_t st) = 0;
   virtual void set_step_height(double h) = 0;
 };
 
@@ -295,6 +310,12 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
     render_launch<real, NJ, TK>(d_twin, (const real*)state_r, state_i, n_envs, env_ids, n_ids, width, height, cam, rgb, st);
   }
 
+  void eval_accumulate(const void* state_r, const int32_t* state_i, int n_envs, const void* reward, const void* rew_terms,
+                       const int32_t* done, double* acc, cudaStream_t st) override {
+    eval_accumulate_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((const real*)state_r, state_i, n_envs, (const real*)reward,
+                                                                               (const real*)rew_terms, done, acc);
+  }
+
   void set_step_height(double h) override {
     if constexpr (Cfg<NJ, TK>::STEP) {   // only the SteppingTask has a curriculum
       model.step_height = (real)h;
@@ -395,6 +416,18 @@ int lhw_sim_render(lhw_sim* s, const void* state_r, const int32_t* state_i, int 
   if (s->bind(st)) return -10;   // leaves the sim's current model in its twin
   const render::Camera cam = render::make_camera(dx, dy, z, distance, azimuth, elevation, fovy, width, height);
   s->render(state_r, state_i, n_envs, env_ids, n_ids, width, height, cam, rgb, st);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_eval_words(void) { return EV_WORDS; }
+
+int lhw_sim_eval_accumulate(lhw_sim* s, const void* state_r, const int32_t* state_i, int n_envs, const void* reward,
+                            const void* rew_terms, const int32_t* done, double* acc, void* stream) {
+  if (!s || !state_r || !state_i || !reward || !rew_terms || !done || !acc) return fail(-1, "null argument");
+  if (n_envs <= 0) return 0;
+  s->eval_accumulate(state_r, state_i, n_envs, reward, rew_terms, done, acc, (cudaStream_t)stream);   // reads no model constants
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

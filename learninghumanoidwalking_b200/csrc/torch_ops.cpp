@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -102,6 +102,22 @@ void sim_render(int64_t sim, const Tensor& state_r, const Tensor& state_i, const
   c10::cuda::CUDAGuard guard(I.device);
   ok(lhw_sim_render(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, env_ids.data_ptr<int32_t>(), (int)k, (int)width, (int)height,
                     dx, dy, z, distance, azimuth, elevation, fovy, rgb.data_ptr<uint8_t>(), stream_of(state_r)), "lhw_sim_render");
+}
+
+void sim_eval_accumulate(int64_t sim, const Tensor& state_r, const Tensor& state_i, const Tensor& reward, const Tensor& rew_terms,
+                         const Tensor& done, Tensor acc) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  check_cuda(reward, "reward", I.real, I.device); check_shape(reward, "reward", {n});
+  check_cuda(rew_terms, "rew_terms", I.real, I.device); check_shape(rew_terms, "rew_terms", {n, 10});
+  check_cuda(done, "done", at::kInt, I.device); check_shape(done, "done", {n});
+  check_cuda(acc, "acc", at::kDouble, I.device); check_shape(acc, "acc", {n, lhw_sim_eval_words()});
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_eval_accumulate(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, reward.data_ptr(), rew_terms.data_ptr(),
+                             done.data_ptr<int32_t>(), acc.data_ptr<double>(), stream_of(state_r)), "lhw_sim_eval_accumulate");
 }
 
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
@@ -304,6 +320,7 @@ TORCH_LIBRARY(lhw, m) {
         "Tensor(i!)? ep_len, Tensor(j!)? ep_rew) -> ()");
   m.def("sim_render(int sim, Tensor state_r, Tensor state_i, Tensor env_ids, int width, int height, float dx, float dy, float z, "
         "float distance, float azimuth, float elevation, float fovy, Tensor(a!) rgb) -> ()");
+  m.def("sim_eval_accumulate(int sim, Tensor state_r, Tensor state_i, Tensor reward, Tensor rew_terms, Tensor done, Tensor(a!) acc) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -333,6 +350,7 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_reset", &sim_reset);
   m.impl("sim_step", &sim_step);
   m.impl("sim_render", &sim_render);
+  m.impl("sim_eval_accumulate", &sim_eval_accumulate);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

@@ -213,6 +213,17 @@ class BatchedHumanoidEnv:
                        "lhw_sim_step")
         return out
 
+    def eval_accumulate(self, acc: torch.Tensor) -> torch.Tensor:
+        """Add the last control step (taken with autoreset=False) to the evaluation accumulators acc, a zero-initialised
+        [N, eval_words()] float64 device tensor, in one launch that only reads the step's outputs and the records (include/lhw_b200.h:
+        lhw_sim_eval_accumulate; rl/evaluation.py names the words)."""
+        _lib.ops().sim_eval_accumulate(self._h.value, self.state_r, self.state_i, self.reward, self.rew_terms, self.done, acc)
+        return acc
+
+    @staticmethod
+    def eval_words() -> int:
+        return _lib.lib().lhw_sim_eval_words()
+
     def bind(self):
         """Upload this env's model constants if another env of the same precision used the constant bank last
         (needed before replaying CUDA graphs that contain lhw_sim_step launches)."""

@@ -4,6 +4,7 @@
     python run_experiment.py train --env jvrc_walk --logdir /tmp/logs --num-procs 4096 --n-itr 100 --seed 0
     python -m torch.distributed.run --nproc-per-node 8 run_experiment.py train --env jvrc_step --num-procs 8192 ...
     python run_experiment.py eval --logdir /tmp/logs [--ep-len 10]
+    python run_experiment.py eval --path RUN_DIR --num-envs 4096 [--precision 32] [--report r.json]
     python run_experiment.py train ... --snapshot; python run_experiment.py resume --path RUN_DIR [--n-itr N]
 
 Same sub-commands and flags as the reference.  What differs underneath: `--num-procs` is the number of parallel environment
@@ -64,7 +65,11 @@ RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a
 EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P, default=None)),
               ("--out-dir", dict(type=_P, default=None, help="write the roll-out as <out-dir>/<actor file stem>.mp4 "
                                                                "(640x480 at 1/control_dt fps; needs OpenCV, the cv2 module)")),
-              ("--ep-len", dict(type=_I, default=10, help="seconds to play")), ("--seed", dict(type=_I, default=None))]
+              ("--ep-len", dict(type=_I, default=10, help="seconds to play")), ("--seed", dict(type=_I, default=None)),
+              # batched evaluation (DESIGN §7.4): N environments, one episode each, statistics gathered on the device
+              ("--num-envs", dict(type=_I, default=None, help="evaluate on N environments at once, env i = Philox env id i")),
+              ("--precision", dict(type=_I, default=None, choices=[32, 64], help="simulator arithmetic of --num-envs (default 64)")),
+              ("--report", dict(type=_P, default=None, help="with --num-envs: write the statistics and per-env arrays as JSON"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -242,8 +247,8 @@ def resume(args):
     return algo.train(env_fn, n_itr, verbose=rank == 0, start_itr=start)
 
 
-def evaluate(args):
-    """Deterministic roll-out of a saved actor on one device environment (the numbers EvaluateEnv would overlay)."""
+def find_actor(args):
+    """The actor file `eval --path / --logdir` names."""
     if args.path is not None:
         if args.path.is_file() and args.path.suffix == ".pt":
             path_to_actor = args.path
@@ -258,6 +263,43 @@ def evaluate(args):
         path_to_actor = get_latest_actor(latest)
     else:
         raise Exception("Must provide either --path or --logdir")
+    return path_to_actor
+
+
+def evaluate_batched(args):
+    """`eval --num-envs N`: the deterministic actor on N environments of the run's env, horizon and YAML, one episode each
+    (rl/evaluation.py), with a table of the outcomes and, with --report, the JSON report."""
+    if args.num_envs < 1:
+        raise SystemExit(f"eval --num-envs {args.num_envs}: needs at least one environment")
+    if args.out_dir is not None:
+        raise SystemExit("eval --out-dir renders one roll-out to video; it cannot be combined with --num-envs")
+    path_to_actor = find_actor(args)
+    print(f"Loading model: {path_to_actor}")
+    with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
+        run_args = pickle.load(f)
+    yaml = run_args.yaml
+    if yaml is not None and Path(path_to_actor.parent, Path(yaml).name).exists():
+        yaml = str(Path(path_to_actor.parent, Path(yaml).name))      # the copy that rode along with the run, as `resume` uses
+    from learninghumanoidwalking_b200.rl.evaluation import evaluate_batched as run
+    from learninghumanoidwalking_b200.rl.policies import install_reference_aliases
+    install_reference_aliases()
+    policy = torch.load(path_to_actor, weights_only=False).cuda().eval()
+    print_system_info(args, training=False)
+    precision = 64 if args.precision is None else args.precision
+    env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
+                                   max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
+    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml))
+    env.close()
+    return report
+
+
+def evaluate(args):
+    """Deterministic roll-out of a saved actor on one device environment (the numbers EvaluateEnv would overlay)."""
+    if args.num_envs is not None:
+        return evaluate_batched(args)
+    if args.precision is not None or args.report is not None:
+        raise SystemExit("eval --precision and --report belong to the batched evaluation: add --num-envs N")
+    path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
         run_args = pickle.load(f)
