@@ -176,6 +176,42 @@ template <class real, class F> LHW_DEV real warp_sum(F f) {
 #endif
 }
 
+// fp64 tensor-core product on one 8x8 tile, a warp collective (called outside LHW_LANES, like warp_sum):
+// D = C + sum_k A_k B_k over KS k-steps of mma.sync m8n8k4 .f64 (A_k 8x4 row-major, B_k 4x8 column-major).
+// Fragment layout (PTX ISA, m8n8k4 .f64): lane l holds A_k[l >> 2][l & 3] = a(l, k), B_k[l & 3][l >> 2] = b(l, k) and
+// C[l >> 2][2 (l & 3) + i] = c(l, i), i = 0, 1; store(l, i, v) receives D at that place.  a and b return 0 for padding.
+// The CPU emulation builds the tiles from the same lambdas and sums C + products in k order; the DMMA's internal rounding
+// order is not specified, so device and host agree to rounding, not bit for bit.
+template <int KS, class FA, class FB, class FC, class FS> LHW_DEV void warp_mma_f64(FA a, FB b, FC c, FS store) {
+#if defined(__CUDA_ARCH__) && !defined(LHW_CPU_EMU)
+  const int l = (int)(threadIdx.x & 31);
+  double d0 = c(l, 0), d1 = c(l, 1);
+#pragma unroll
+  for (int k = 0; k < KS; k++) {
+    const double ak = a(l, k), bk = b(l, k);
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
+                 : "+d"(d0), "+d"(d1) : "d"(ak), "d"(bk));
+  }
+  store(l, 0, d0);
+  store(l, 1, d1);
+#else
+  double A[KS][8][4], B[KS][4][8], D[8][8];
+  for (int l = 0; l < 32; ++l) {
+    for (int k = 0; k < KS; k++) {
+      A[k][l >> 2][l & 3] = a(l, k);
+      B[k][l & 3][l >> 2] = b(l, k);
+    }
+    for (int i = 0; i < 2; i++) D[l >> 2][2 * (l & 3) + i] = c(l, i);
+  }
+  for (int r = 0; r < 8; r++)
+    for (int col = 0; col < 8; col++)
+      for (int k = 0; k < KS; k++)
+        for (int kk = 0; kk < 4; kk++) D[r][col] += A[k][r][kk] * B[k][kk][col];
+  for (int l = 0; l < 32; ++l)
+    for (int i = 0; i < 2; i++) store(l, i, D[l >> 2][2 * (l & 3) + i]);
+#endif
+}
+
 // warp ballot of a per-lane predicate; bit helpers (the CPU emulation evaluates the predicate lane by lane)
 template <class F> LHW_DEV unsigned warp_ballot(F f) {
 #if defined(__CUDA_ARCH__) && !defined(LHW_CPU_EMU)
@@ -725,6 +761,83 @@ template <class real> LHW_DEV real floss_force(real D, real lim, real fl, real x
   if (x >= lim) { *curv = 0; return -fl; }
   *curv = D;
   return -D * x;
+}
+
+// P10 (e, second half) and (f) of the fp64 kernels on the fp64 tensor cores (mma.sync m8n8k4): T_f = Af S_f, then
+// H = M + sum_f S_f' T_f + the limit / friction-loss diagonal, on the arrow pattern.  Af must be complete (after an LHW_SYNC);
+// H is complete after the next LHW_SYNC.  Out of line (like arrow_factor_solve), so that its fragment addressing does not add
+// to substep's live registers.
+// Padding: only the padded k of BOTH operands are zeroed.  The padded rows and columns of a tile repeat the block's last row or
+// column and reach only entries of D that are never stored, so each lane needs one predicate for its fragments,
+// (l & 3) < 2, and every read stays inside its block.
+template <class real, int NJ, int TK> LHW_DEVNI void newton_hessian_f64(Work<real, NJ, TK>& w) {
+  LHW_ASSUME_SHARED(&w);
+  constexpr int NA = 6 + NJ;
+  constexpr bool FLOSS = Cfg<NJ, TK>::FLOSS;
+  const double* const S = &w.S[0][0];
+  // k-step k of a 6-long sum: lane l holds term 4 k + (l & 3) of row / column l >> 2 of a row-major block of `rows` rows and
+  // stride 6
+  const auto frag6 = [](const double* p, int rows, int l, int k) {
+    return k && (l & 3) >= 2 ? 0.0 : p[m_min(l >> 2, rows - 1) * 6 + (l & 3) + 4 * k];
+  };
+  // C fragment entry of a row-major rows x cols block
+  const auto cfrag = [](const double* p, int rows, int cols, int l, int i) {
+    return p[m_min(l >> 2, rows - 1) * cols + m_min(2 * (l & 3) + i, cols - 1)];
+  };
+  // T_f in two tiles per foot, the root dofs and the foot's chain dofs, 2 k-steps each; T_f = 0 without contacts.
+  // T_f goes through w.T[foot][dof][component]: the C fragment of this product is not the B fragment of the next one
+#pragma unroll
+  for (int f = 0; f < 2; f++) {
+    if (w.ncon[f]) {
+#pragma unroll
+      for (int n = 0; n < 2; n++)
+        warp_mma_f64<2>([&](int l, int k) { return frag6(&w.Af[f][0][0], 6, l, k); },
+                        [&](int l, int k) { return frag6(S + 6 * (n ? 6 + f * NJ : 0), n ? NJ : 6, l, k); },
+                        [](int, int) { return 0.0; },
+                        [&](int l, int i, double v) {
+                          const int a = l >> 2, j = 2 * (l & 3) + i;
+                          if (a < 6 && j < (n ? NJ : 6)) w.T[f][6 * n + j][a] = v;
+                        });
+    } else {
+      LHW_LANES(l) { LHW_STRIDED(it, l, NA * 6) (&w.T[f][0][0])[it] = 0; }
+    }
+  }
+  LHW_SYNC();
+  // H as five tiles: the root block (both feet in one chain of 4 k-steps) and per chain the coupling block (root rows x chain
+  // columns) and the chain block (2 k-steps each).  A fragments: S' of the root dofs (root and coupling tiles) or of the chain
+  // dofs; B: T.  Only the lower triangles the factorisation reads are stored
+  const double* const T = &w.T[0][0][0];
+  const auto s_root = [&](int l, int k) { return frag6(S, 6, l, k & 1); };
+  warp_mma_f64<4>(s_root, [&](int l, int k) { return frag6(T + (k >> 1) * NA * 6, 6, l, k & 1); },
+                  [&](int l, int i) { return cfrag(&w.M.r[0][0], 6, 6, l, i); },
+                  [&](int l, int i, double v) {
+                    const int r = l >> 2, t = 2 * (l & 3) + i;
+                    if (r < 6 && t <= r) w.H.r[r][t] = v;
+                  });
+#pragma unroll
+  for (int ch = 0; ch < 2; ch++) {
+    const auto t_chain = [&](int l, int k) { return frag6(T + (ch * NA + 6) * 6, NJ, l, k); };
+    warp_mma_f64<2>(s_root, t_chain, [&](int l, int i) { return cfrag(&w.M.x[ch][0][0], 6, NJ, l, i); },
+                    [&](int l, int i, double v) {
+                      const int j = l >> 2, k = 2 * (l & 3) + i;
+                      if (j < 6 && k < NJ) w.H.x[ch][j][k] = v;
+                    });
+    warp_mma_f64<2>([&](int l, int k) { return frag6(S + 6 * (6 + ch * NJ), NJ, l, k); }, t_chain,
+                    [&](int l, int i) { return cfrag(&w.M.c[ch][0][0], NJ, NJ, l, i); },
+                    [&](int l, int i, double v) {
+                      const int k = l >> 2, t = 2 * (l & 3) + i;
+                      if (k < NJ && t <= k) {
+                        if (k == t && w.lside[ch * NJ + k] && w.ljar[ch * NJ + k] < 0) v += w.lD[ch * NJ + k];
+                        if constexpr (FLOSS) {
+                          if (k == t) {
+                            const real xj = w.fjar[ch * NJ + k], lim = w.flim[ch * NJ + k];
+                            if (xj > -lim && xj < lim) v += w.fD[ch * NJ + k];
+                          }
+                        }
+                        w.H.c[ch][k][t] = v;
+                      }
+                    });
+  }
 }
 
 // ================================================================= one physics substep (mujoco.mj_step)
@@ -1430,6 +1543,9 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
       }
     }
     LHW_SYNC();
+    if constexpr (sizeof(real) == 8) {
+      newton_hessian_f64<real, NJ, TK>(w);
+    } else {
     // ... and T_f = Af S_f (per foot, per ancestor dof, per component)
     LHW_LANES(l) {
       for (int it = l; it < 2 * NA * 6; it += 32) {
@@ -1468,6 +1584,7 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
           w.H.c[ch][k][t] = acc;
         }
       }
+    }
     }
     LHW_SYNC();
     arrow_factor_solve<real, NJ, TK>(w, w.sdir);

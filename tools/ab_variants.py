@@ -27,6 +27,8 @@ BUILDS = {
     # warm starts of the Newton solve, screened with tools/newton_census.py (DESIGN.md §4.1): the extrapolated warm start won on
     # every workload and regime and is now the kernel; the active-set warm start (first Hessian from the previous solve's final
     # active set), alone or with it, raised the block maximum everywhere and was deleted before any GPU timing
+    # the Newton Hessian (T_f, H) on the fp64 tensor cores is now the fp64 kernel (DESIGN.md §4.1); the root Schur complement as one
+    # DMMA tile timed x1.012 on top of it but made ptxas spill in reset_kernel<double, 6, 0>, and was dropped
 }
 # (build, env knobs) timed on (model, precision, n_envs); runs with knobs only time the headline workload
 RUNS = [
