@@ -102,6 +102,16 @@ int lhw_sim_eval_words(void);
 int lhw_sim_eval_accumulate(lhw_sim* sim, const void* state_r, const int32_t* state_i, int n_envs, const void* reward,
                             const void* rew_terms, const int32_t* done, double* acc, void* stream);
 
+/* lhw_sim_push: root-velocity pushes (DESIGN.md §7.5; legged_gym's push_robots, the reference has none).  One launch over n envs
+ * that adds Rz(psi) (dx, dy) to qvel[0:2] of the records state_r it pushes (world frame; psi = heading of qpos[3:7], (dx, dy) in
+ * the heading frame: x forward, y to the robot's left) and writes nothing else.  state_i is only read.
+ * Explicit mode, d != NULL: d [n, 2] in the sim's precision; rows that are exactly 0 are skipped (ended, vel, interval unused).
+ * Random mode, d == NULL: after an lhw_sim_step over the same envs; an env whose ended [n] flag is 0 is pushed when
+ * randint(u0, interval_steps) == 0 for u = philox(seed, first_env_id + i, rng_ctr, 70), by vel (2 u01(u1) - 1, 2 u01(u2) - 1).
+ * vel must be finite and >= 0, interval_steps >= 1.  Reads no model constants. */
+int lhw_sim_push(lhw_sim* sim, void* state_r, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                 const int32_t* ended, double vel, int interval_steps, const void* d, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

@@ -2520,4 +2520,45 @@ LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward,
   if (done) acc[EV_DONE] = 1;
 }
 
+// ================================================================= root-velocity pushes (lhw_sim_push, DESIGN.md §7.5)
+// legged_gym's push_robots: a horizontal velocity impulse on the root, qvel[0:2] (world frame) += Rz(psi) (dx, dy), with psi the
+// heading (yaw) of qpos[3:7] and (dx, dy) in the heading frame (x forward, y to the robot's left).  Every link gets the same dv;
+// joint velocities are unchanged.  Nothing else of the record is written, and nothing of an env that is not pushed.
+// The random pushes draw on their own Philox stream at the env's event counter, which they only read.  The step and reset
+// bodies above draw on streams 0-5, 8-13, 16-35, 40-48, 50-54 and 60-64, so with pushes off every trajectory is unchanged.
+constexpr uint32_t PUSH_STREAM = 70;
+
+// One env's push; returns 1 when it was pushed.  Explicit mode (d != nullptr): (dx, dy) = (d[0], d[1]), skipped when both are
+// exactly 0.  Random mode (d == nullptr): skipped when `ended` (the env was just reset); else pushed with probability 1/interval
+// by u = philox(seed, env_id, rng_ctr, PUSH_STREAM): randint(u[0], interval) == 0, then (dx, dy) = vel (2 u01(u[1]) - 1,
+// 2 u01(u[2]) - 1).  The arithmetic is float64 at either precision; the sum is rounded once to the record's precision.
+template <class real, int NJ, int TK>
+LHW_DEV int push_env(real* sr, const int32_t* si, uint32_t seed, uint32_t env_id, int32_t ended, double vel, int interval,
+                     const real* d) {
+  using A = RecordAt<real, NJ, TK>;
+  double dx, dy;
+  if (d) {
+    if (d[0] == 0 && d[1] == 0) return 0;
+    dx = (double)d[0];
+    dy = (double)d[1];
+  } else {
+    if (ended) return 0;
+    uint32_t u[4];
+    philox(seed, env_id, (uint32_t)si[4], PUSH_STREAM, u);   // si[4]: rng_ctr (load_state)
+    if (randint(u[0], interval) != 0) return 0;
+    dx = vel * (2 * u01<double>(u[1]) - 1);
+    dy = vel * (2 * u01<double>(u[2]) - 1);
+  }
+  // heading: the first column of the root's rotation matrix (the quaternion normalised as eval_accumulate_env does), projected on
+  // the ground plane; (c, s) = (cos psi, sin psi)
+  const double qw = (double)sr[A::QPOS + 3], x = (double)sr[A::QPOS + 4], y = (double)sr[A::QPOS + 5], z = (double)sr[A::QPOS + 6];
+  const double q2 = 2 / (qw * qw + x * x + y * y + z * z);
+  const double r00 = 1 - q2 * (y * y + z * z), r10 = q2 * (x * y + qw * z);
+  const double h = m_sqrt(r00 * r00 + r10 * r10);
+  const double c = h > 0 ? r00 / h : 1, s = h > 0 ? r10 / h : 0;
+  sr[A::QVEL + 0] = (real)((double)sr[A::QVEL + 0] + (c * dx - s * dy));
+  sr[A::QVEL + 1] = (real)((double)sr[A::QVEL + 1] + (s * dx + c * dy));
+  return 1;
+}
+
 }  // namespace lhw

@@ -185,6 +185,17 @@ __global__ void __launch_bounds__(256) eval_accumulate_kernel(const real* __rest
                                     rew_terms + (size_t)env * NREW, done[env], acc + (size_t)env * EV_WORDS);
 }
 
+// root-velocity pushes: one thread per env, qvel[0:2] of the pushed envs written in place, nothing else (sim_core.h push_env)
+template <class real, int NJ, int TK>
+__global__ void __launch_bounds__(256) push_kernel(real* __restrict__ state_r, const int32_t* __restrict__ state_i, int n_envs,
+                                                  uint32_t seed, uint32_t first_id, const int32_t* __restrict__ ended, double vel,
+                                                  int interval, const real* __restrict__ d) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= n_envs) return;
+  push_env<real, NJ, TK>(state_r + (size_t)env * Dims<real, NJ, TK>::NSTATE_R, state_i + (size_t)env * NSTATE_I, seed, first_id + env,
+                         ended ? ended[env] : 0, vel, interval, d ? d + 2 * (size_t)env : nullptr);
+}
+
 }  // namespace
 
 // what every sim has, whichever its variant; SimOf<real, NJ, TK> holds its model and launches its kernels
@@ -203,6 +214,8 @@ struct lhw_sim {
                       int height, const render::Camera& cam, uint8_t* rgb, cudaStream_t st) = 0;
   virtual void eval_accumulate(const void* state_r, const int32_t* state_i, int n_envs, const void* reward, const void* rew_terms,
                                const int32_t* done, double* acc, cudaStream_t st) = 0;
+  virtual void push(void* state_r, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* ended,
+                    double vel, int interval, const void* d, cudaStream_t st) = 0;
   virtual void set_step_height(double h) = 0;
 };
 
@@ -314,6 +327,12 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
                        const int32_t* done, double* acc, cudaStream_t st) override {
     eval_accumulate_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((const real*)state_r, state_i, n_envs, (const real*)reward,
                                                                                (const real*)rew_terms, done, acc);
+  }
+
+  void push(void* state_r, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* ended, double vel,
+            int interval, const void* d, cudaStream_t st) override {
+    push_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, ended, vel,
+                                                                    interval, (const real*)d);
   }
 
   void set_step_height(double h) override {
@@ -428,6 +447,18 @@ int lhw_sim_eval_accumulate(lhw_sim* s, const void* state_r, const int32_t* stat
   if (!s || !state_r || !state_i || !reward || !rew_terms || !done || !acc) return fail(-1, "null argument");
   if (n_envs <= 0) return 0;
   s->eval_accumulate(state_r, state_i, n_envs, reward, rew_terms, done, acc, (cudaStream_t)stream);   // reads no model constants
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_push(lhw_sim* s, void* state_r, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                 const int32_t* ended, double vel, int interval_steps, const void* d, void* stream) {
+  if (!s || !state_r || !state_i || (!d && !ended)) return fail(-1, "null argument");
+  if (!d && !(vel >= 0 && vel <= 1e30)) return fail(-2, "push velocity must be finite and non-negative");
+  if (!d && interval_steps < 1) return fail(-2, "push interval must be at least one control step");
+  if (n_envs <= 0) return 0;
+  s->push(state_r, state_i, n_envs, seed, first_env_id, ended, vel, interval_steps, d, (cudaStream_t)stream);   // no model constants
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

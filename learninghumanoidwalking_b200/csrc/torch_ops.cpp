@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -12,6 +12,8 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
 #include <torch/library.h>
+
+#include <cmath>
 
 #include "../../include/lhw_b200.h"
 
@@ -118,6 +120,27 @@ void sim_eval_accumulate(int64_t sim, const Tensor& state_r, const Tensor& state
   c10::cuda::CUDAGuard guard(I.device);
   ok(lhw_sim_eval_accumulate(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, reward.data_ptr(), rew_terms.data_ptr(),
                              done.data_ptr<int32_t>(), acc.data_ptr<double>(), stream_of(state_r)), "lhw_sim_eval_accumulate");
+}
+
+void sim_push(int64_t sim, Tensor state_r, const Tensor& state_i, int64_t seed, int64_t first_env_id, const OptTensor& ended, double vel,
+              int64_t interval_steps, const OptTensor& d) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  TORCH_CHECK(d.has_value() != ended.has_value(), "lhw: sim_push takes either d (explicit pushes) or ended (random pushes)");
+  if (d) { check_cuda(*d, "d", I.real, I.device); check_shape(*d, "d", {n, 2}); }
+  if (ended) {
+    check_cuda(*ended, "ended", at::kInt, I.device); check_shape(*ended, "ended", {n});
+    TORCH_CHECK(std::isfinite(vel) && vel >= 0, "lhw: push velocity must be finite and non-negative, got ", vel);
+    TORCH_CHECK(interval_steps >= 1 && interval_steps <= INT32_MAX, "lhw: push interval must be at least one control step, got ",
+                interval_steps);
+  }
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_push(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                  ended ? ended->data_ptr<int32_t>() : nullptr, vel, (int)interval_steps, d ? d->data_ptr() : nullptr, stream_of(state_r)),
+     "lhw_sim_push");
 }
 
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
@@ -321,6 +344,8 @@ TORCH_LIBRARY(lhw, m) {
   m.def("sim_render(int sim, Tensor state_r, Tensor state_i, Tensor env_ids, int width, int height, float dx, float dy, float z, "
         "float distance, float azimuth, float elevation, float fovy, Tensor(a!) rgb) -> ()");
   m.def("sim_eval_accumulate(int sim, Tensor state_r, Tensor state_i, Tensor reward, Tensor rew_terms, Tensor done, Tensor(a!) acc) -> ()");
+  m.def("sim_push(int sim, Tensor(a!) state_r, Tensor state_i, int seed, int first_env_id, Tensor? ended, float vel, int interval_steps, "
+        "Tensor? d) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -351,6 +376,7 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_step", &sim_step);
   m.impl("sim_render", &sim_render);
   m.impl("sim_eval_accumulate", &sim_eval_accumulate);
+  m.impl("sim_push", &sim_push);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

@@ -36,6 +36,17 @@ H1_WALK_MIRRORED_OBS = [-0.1, 1, -2, 3, -4,
 H1_WALK_MIRRORED_ACTS = [-5, -6, 7, 8, 9, -0.1, -1, 2, 3, 4]
 
 
+def push_interval_steps(push_vel: float, push_interval: float, dt: float) -> int:
+    """The random pushes' mean interval in control steps, round(push_interval / dt), after refusing a push speed that is
+    negative or not finite and an interval that is not finite or shorter than one control step (DESIGN.md §7.5)."""
+    push_vel, push_interval = float(push_vel), float(push_interval)
+    if not (np.isfinite(push_vel) and push_vel >= 0):
+        raise ValueError(f"push_vel must be a finite speed >= 0 m/s, got {push_vel}")
+    if not (np.isfinite(push_interval) and push_interval >= dt):
+        raise ValueError(f"push_interval must be a finite number of seconds of at least one control step ({dt} s), got {push_interval}")
+    return int(round(push_interval / dt))
+
+
 class _Robot(SimpleNamespace):
     """The attributes the trainer reads / writes on `env.robot` (robots/robot_base.py:35, run_experiment.py:123-125).
     Writing `iteration_count` (rl/workers/rollout_worker.py:95) drives the SteppingTask's height curriculum."""
@@ -51,7 +62,7 @@ class BatchedHumanoidEnv:
                  first_env_id: int = 0, device: int | torch.device | None = None, max_traj_len: int = 400,
                  tolerance: float | None = None, max_iter: int | None = None, observation_noise: bool = True,
                  domain_randomization: bool = True, init_noise: bool = True, pd_gain_randomization: float = 0.0,
-                 iteration_count: float = float("inf"), path_to_yaml=None):
+                 iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0):
         if not torch.cuda.is_available():
             raise _lib.LhwError("BatchedHumanoidEnv needs a CUDA device (no CPU fallback on the rollout path)")
         if device is None:
@@ -67,6 +78,9 @@ class BatchedHumanoidEnv:
             from .config import apply_config, load_yaml
             self.mj = apply_config(self.mj, load_yaml(path_to_yaml))
         self._iteration_count = float(iteration_count)
+        # random root-velocity pushes after every control step (DESIGN.md §7.5): off at push_vel == 0, and then nothing is launched
+        self.push_vel, self.push_interval = float(push_vel), float(push_interval)
+        self.push_interval_steps = push_interval_steps(push_vel, push_interval, self.mj["cfg"]["control_dt"])
         if tolerance is None and precision == 32:
             tolerance = 1e-6  # fp32 cannot reach the reference's 1e-10; gradient floor is ~1e-6 of the force scale
         flat = pack_model(self.mj, tolerance=tolerance, max_iter=max_iter, observation_noise=observation_noise,
@@ -178,6 +192,7 @@ class BatchedHumanoidEnv:
             _lib.ops().sim_step(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, actions, self.max_traj_len,
                                 bool(autoreset), self.obs, self.term_obs, self.reward, self.rew_terms, self.done, self.ended,
                                 self.ep_len, self.ep_rew)
+            self._push_random(0, self.num_envs)
             return self.obs, self.reward, self.done, self.ended
         assert actions.shape == (self.num_envs, self.act_dim), actions.shape
         L = _lib.lib()
@@ -188,6 +203,7 @@ class BatchedHumanoidEnv:
                                       self.rew_terms.data_ptr(), self.done.data_ptr(), self.ended.data_ptr(),
                                       self.ep_len.data_ptr(), self.ep_rew.data_ptr(), _lib.current_stream_ptr()),
                        "lhw_sim_step")
+        self._push_random(0, self.num_envs)
         return self.obs, self.reward, self.done, self.ended
 
     def step_slice(self, lo: int, hi: int, actions: torch.Tensor, autoreset: bool = True):
@@ -202,6 +218,7 @@ class BatchedHumanoidEnv:
             _lib.ops().sim_step(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
                                 self.max_traj_len, bool(autoreset), out[0], self.term_obs[sl], out[1], self.rew_terms[sl], out[2], out[3],
                                 self.ep_len[sl], self.ep_rew[sl])
+            self._push_random(lo, hi)
             return out
         assert actions.shape == (hi - lo, self.act_dim), actions.shape
         with torch.cuda.device(self.device):
@@ -211,7 +228,23 @@ class BatchedHumanoidEnv:
                                                self.rew_terms[sl].data_ptr(), out[2].data_ptr(), out[3].data_ptr(),
                                                self.ep_len[sl].data_ptr(), self.ep_rew[sl].data_ptr(), _lib.current_stream_ptr()),
                        "lhw_sim_step")
+        self._push_random(lo, hi)
         return out
+
+    def _push_random(self, lo: int, hi: int) -> None:
+        """The random pushes of environments [lo, hi) after their control step, on the same stream; none at push_vel == 0.
+        An env that the step ended (and so reset) is not pushed; the draws are keyed by the env's Philox id and event counter."""
+        if self.push_vel > 0:
+            _lib.ops().sim_push(self._h.value, self.state_r[lo:hi], self.state_i[lo:hi], self.seed, self.first_env_id + lo,
+                                self.ended[lo:hi], self.push_vel, self.push_interval_steps, None)
+
+    def push(self, d: torch.Tensor) -> None:
+        """Push every environment once, now: d [N, 2] holds each one's velocity change (dx, dy) in m/s in its heading frame (x
+        forward, y to the robot's left), added to the root's world-frame qvel[0:2] after rotation by the heading.  Rows that are
+        exactly zero are left untouched, and nothing else of any record changes (include/lhw_b200.h: lhw_sim_push)."""
+        if d.dtype != self.dtype or not d.is_contiguous() or d.device != self.device:
+            d = d.to(device=self.device, dtype=self.dtype).contiguous()
+        _lib.ops().sim_push(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, None, 0.0, 1, d)
 
     def eval_accumulate(self, acc: torch.Tensor) -> torch.Tensor:
         """Add the last control step (taken with autoreset=False) to the evaluation accumulators acc, a zero-initialised

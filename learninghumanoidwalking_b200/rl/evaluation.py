@@ -5,6 +5,11 @@ max_traj_len control steps: each environment's first episode is one sample.  Aft
 (BatchedHumanoidEnv.eval_accumulate, csrc/sim_core.h eval_accumulate_env) adds it to a per-env float64 accumulator record on the
 device; the host reads the records once, at the end.  The control step (actor forward, step, accumulate) is captured as one
 CUDA graph after an eager first step and replayed, as the rollout worker does.
+
+The push-recovery sweep (`eval --num-envs N --push-speeds ...`, DESIGN.md §7.5) pushes every environment once, after control step
+K = round(push_at / dt), between two replays of the same graph: env i gets the speed and heading-frame direction of grid cell
+i mod (speeds x directions).  A fallen env is not pushed (a device-side `where` on its ended-by-done word), and the statistics come
+from the same accumulator words: fell before the push (EV_DONE set and EV_LEN <= K), survived (EV_DONE clear at the horizon).
 """
 from __future__ import annotations
 
@@ -19,14 +24,38 @@ MODES = ("STANDING", "INPLACE", "FORWARD")     # WalkingTask's modes, in the ord
 TRACKED = ("jvrc_walk", "jvrc_walk_terrain", "h1_walk", "h1")   # h1: its StandingTask, against zero references
 
 
+def push_grid(n: int, speeds, directions: int):
+    """Per env (speed m/s, direction in degrees) of the sweep: env i is cell c = i mod (S D), with speed speeds[c // D] and
+    direction 360 (c mod D) / D in its heading frame (0 forward, 90 towards the robot's left)."""
+    c = np.arange(n) % (len(speeds) * directions)
+    return np.asarray(speeds, dtype=np.float64)[c // directions], 360.0 * (c % directions) / directions
+
+
+def push_vectors(speed: np.ndarray, dir_deg: np.ndarray) -> np.ndarray:
+    """[N, 2] heading-frame velocity changes (dx, dy) of the sweep."""
+    th = np.deg2rad(dir_deg)
+    return np.stack((speed * np.cos(th), speed * np.sin(th)), axis=1)
+
+
 @torch.no_grad()
-def rollout(env, policy, steps: int, graph: bool = True) -> torch.Tensor:
+def rollout(env, policy, steps: int, graph: bool = True, push=None) -> torch.Tensor:
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
-    [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order)."""
+    [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
+    push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
+    change d [N, 2] (BatchedHumanoidEnv.push); with push=None nothing but the control steps is launched."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
     acc = torch.zeros(env.num_envs, WORDS, dtype=torch.float64, device=env.device)
     state = env.reset().float().clone()
+    push_k, push_d = push if push is not None else (None, None)
+    if push is not None:
+        if not 1 <= push_k < steps:
+            raise ValueError(f"the push must come after control step 1..{steps - 1}, got {push_k}")
+        push_d = torch.as_tensor(push_d).to(device=env.device, dtype=env.dtype).reshape(env.num_envs, 2).contiguous()
+
+    def after(t):     # after control step t (1-based)
+        if t == push_k:
+            env.push(torch.where(acc[:, DONE:DONE + 1] != 0, torch.zeros_like(push_d), push_d))   # the fallen stay where they lie
 
     def body():
         a = policy(state, deterministic=True)
@@ -35,8 +64,9 @@ def rollout(env, policy, steps: int, graph: bool = True) -> torch.Tensor:
         state.copy_(obs.float())
 
     if not graph or steps <= 1:
-        for _ in range(steps):
+        for t in range(steps):
             body()
+            after(t + 1)
         return acc
     cur = torch.cuda.current_stream(env.device)
     s = torch.cuda.Stream(device=env.device)
@@ -46,9 +76,11 @@ def rollout(env, policy, steps: int, graph: bool = True) -> torch.Tensor:
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, stream=s):
             body()     # capturing does not execute: the replays run steps 2..steps
+        after(1)
         env.bind()
-        for _ in range(steps - 1):
+        for t in range(2, steps + 1):
             g.replay()
+            after(t)
     cur.wait_stream(s)
     return acc
 
@@ -93,6 +125,41 @@ def per_env(acc: np.ndarray, env_name: str, reward_names) -> dict:
     return out
 
 
+def push_summary(acc: np.ndarray, speed: np.ndarray, dir_deg: np.ndarray, speeds, directions: int, push_at: float,
+                 push_step: int) -> dict:
+    """The sweep's outcome per cell (speed x direction) and per speed: n, fell before the push, alive at the push, survived to the
+    horizon, and survival = survived / alive at the push (None when no env was alive)."""
+    fell = acc[:, DONE] != 0
+    before = fell & (acc[:, LEN] <= push_step)
+    surv = lambda s, a: float(s / a) if a else None
+    cells = []
+    for si, v in enumerate(speeds):
+        for k in range(directions):
+            m = (speed == float(v)) & (dir_deg == 360.0 * k / directions)
+            n, b, ok = int(m.sum()), int((m & before).sum()), int((m & ~fell).sum())
+            cells.append(dict(speed=float(v), direction_deg=360.0 * k / directions, n=n, fell_before_push=b, alive_at_push=n - b,
+                              survived=ok, survival=surv(ok, n - b)))
+    per_speed = []
+    for v in speeds:
+        cs = [c for c in cells if c["speed"] == float(v)]
+        alive, ok = sum(c["alive_at_push"] for c in cs), sum(c["survived"] for c in cs)
+        per_speed.append(dict(speed=float(v), alive_at_push=alive, survived=ok, survival=surv(ok, alive)))
+    return dict(speeds=[float(v) for v in speeds], directions_deg=[360.0 * k / directions for k in range(directions)],
+                push_at=float(push_at), push_step=int(push_step), cells=cells, per_speed=per_speed)
+
+
+def format_push_table(p: dict) -> str:
+    f = lambda v: "    -" if v is None else f"{v:5.3f}"
+    lines = [f"  push recovery: one push after control step {p['push_step']} ({p['push_at']} s); survival = survived to the horizon / "
+             "alive at the push",
+             "    speed m/s \\ direction deg " + "".join(f"{d:>7.0f}" for d in p["directions_deg"]) + "    all"]
+    nd = len(p["directions_deg"])
+    for i, ps in enumerate(p["per_speed"]):
+        row = p["cells"][i * nd:(i + 1) * nd]
+        lines.append(f"    {ps['speed']:>27.3f} " + "".join(f"  {f(c['survival'])}" for c in row) + f"  {f(ps['survival'])}")
+    return "\n".join(lines)
+
+
 def format_table(s: dict, max_traj_len: int) -> str:
     L = s["length"]
     lines = [f"{s['num_envs']} environments, one episode each, horizon {max_traj_len} control steps",
@@ -113,14 +180,25 @@ def format_table(s: dict, max_traj_len: int) -> str:
     return "\n".join(lines)
 
 
-def evaluate_batched(policy, env, out_report=None, meta: dict | None = None) -> dict:
+def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
-    out_report, write the JSON report (meta + summary + per-env arrays).  Returns the report."""
-    acc = rollout(env, policy, env.max_traj_len).cpu().numpy()
+    out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
+    push-recovery sweep, with its table and `summary.push`.  Returns the report."""
+    sweep = None
+    if push is not None:
+        k = int(round(push["push_at"] / env.dt))
+        speed, dir_deg = push_grid(env.num_envs, push["speeds"], push["directions"])
+        sweep = (k, push_vectors(speed, dir_deg))
+    acc = rollout(env, policy, env.max_traj_len, push=sweep).cpu().numpy()
     summary = summarize(acc, env.model_name, env.reward_names)
+    pe = per_env(acc, env.model_name, env.reward_names)
     print(format_table(summary, env.max_traj_len))
+    if push is not None:
+        summary["push"] = push_summary(acc, speed, dir_deg, push["speeds"], push["directions"], push["push_at"], k)
+        pe.update(push_speed=speed.tolist(), push_dir_deg=dir_deg.tolist())
+        print(format_push_table(summary["push"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
-                  max_traj_len=env.max_traj_len, summary=summary, per_env=per_env(acc, env.model_name, env.reward_names))
+                  max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:
         with open(out_report, "w") as f:
             json.dump(report, f, indent=1)

@@ -17,6 +17,12 @@ Artefacts keep the reference's names and format: `<logdir>/<timestamp>_<env>/exp
 `critic_<itr>.pt` (whole pickled modules, rl/utils/checkpointer.py:51-83); `train --imitate PATH` also keeps a copy of the
 teacher as `teacher.pt` (DESIGN §7.2).  `train --schedule adaptive [--desired-kl 0.01]` adapts the learning rate to the policy's
 KL after every minibatch (rsl_rl's schedule, DESIGN §7.3); the rate is printed and logged as `Train/learning_rate`.
+`train --push-vel V [--push-interval S]` adds legged_gym-style random pushes to every environment: about every S seconds (default
+15) an env's root gets a horizontal velocity change of up to V m/s per axis of its heading frame (DESIGN §7.5).  The periodic
+evaluation batches run on the training env and see the pushes too; `resume` rebuilds the env with the run's values, and a run
+recorded without them has none.  `eval --num-envs N --push-speeds 0,0.5,1,1.5 [--push-directions 8] [--push-at 2.0]` pushes each
+env once, at --push-at seconds, with the speed and direction of its cell of the grid (env i: cell i mod speeds x directions), and
+prints the survival of each cell; the batched evaluation never gets the training pushes.
 """
 import argparse
 import os
@@ -59,6 +65,8 @@ TRAIN_FLAGS = [
     ("--schedule", dict(type=_S, default="fixed", choices=["fixed", "adaptive"],
                         help="learning rate: fixed at --lr, or adaptive: starts at --lr and follows the minibatch KL (DESIGN §7.3)")),
     ("--desired-kl", dict(type=_F, default=0.01, help="target KL of --schedule adaptive")),
+    ("--push-vel", dict(type=_F, default=0.0, help="random root-velocity pushes of up to V m/s per horizontal axis (0: off; DESIGN §7.5)")),
+    ("--push-interval", dict(type=_F, default=15.0, help="mean seconds between two random pushes of an env")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -69,7 +77,11 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
               # batched evaluation (DESIGN §7.4): N environments, one episode each, statistics gathered on the device
               ("--num-envs", dict(type=_I, default=None, help="evaluate on N environments at once, env i = Philox env id i")),
               ("--precision", dict(type=_I, default=None, choices=[32, 64], help="simulator arithmetic of --num-envs (default 64)")),
-              ("--report", dict(type=_P, default=None, help="with --num-envs: write the statistics and per-env arrays as JSON"))]
+              ("--report", dict(type=_P, default=None, help="with --num-envs: write the statistics and per-env arrays as JSON")),
+              # push-recovery sweep of the batched evaluation (DESIGN §7.5)
+              ("--push-speeds", dict(type=_S, default=None, help="with --num-envs: comma-separated push speeds in m/s, e.g. 0,0.5,1,1.5")),
+              ("--push-directions", dict(type=_I, default=None, help="push directions, evenly spaced from forward (default 8)")),
+              ("--push-at", dict(type=_F, default=None, help="seconds into the episode of the one push (default 2.0)"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -90,6 +102,9 @@ def print_system_info(args, training=True):
                      ("Learning rate", args.lr), ("Max trajectory length", args.max_traj_len), ("Iterations", args.n_itr),
                      ("Seed", args.seed)):
             print(f"{k}: {v}")
+        push_vel = getattr(args, "push_vel", 0.0)
+        print(f"Random pushes: up to {push_vel} m/s about every {getattr(args, 'push_interval', 15.0)} s" if push_vel > 0
+              else "Random pushes: off")
     print("=" * 60)
 
 
@@ -136,7 +151,8 @@ def make_env_fn(args, rank, world, local):
     first, n_local = env_shard(rank, world, args.num_procs)
     seed = args.seed if args.seed is not None else 0
     env_fn = partial(Env, n_local, precision=args.precision, seed=seed, first_env_id=first, device=local,
-                     max_traj_len=args.max_traj_len, path_to_yaml=args.yaml)
+                     max_traj_len=args.max_traj_len, path_to_yaml=args.yaml, push_vel=getattr(args, "push_vel", 0.0),
+                     push_interval=getattr(args, "push_interval", 15.0))   # an experiment.pkl without them: no pushes
     _env = env_fn()
     if not args.no_mirror:
         try:
@@ -164,8 +180,25 @@ def check_schedule(args):
                          "baseline exchange, which has no adaptive schedule")
 
 
+def check_push(args):
+    """Refuse random-push flags the env would refuse, before any environment or run directory exists."""
+    from learninghumanoidwalking_b200.envs.batched_env import push_interval_steps
+    from learninghumanoidwalking_b200.model import load_model
+    push_vel, push_interval = getattr(args, "push_vel", 0.0), getattr(args, "push_interval", 15.0)
+    import_env(args.env)
+    mj = load_model(args.env)
+    if args.yaml is not None:
+        from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
+        mj = apply_config(mj, load_yaml(args.yaml))
+    try:
+        push_interval_steps(push_vel, push_interval, mj["cfg"]["control_dt"])
+    except ValueError as e:
+        raise SystemExit(f"train --push-vel {push_vel} --push-interval {push_interval}: {e}")
+
+
 def run_experiment(args):
     from learninghumanoidwalking_b200.rl import PPO
+    check_push(args)
     rank, world, local = _dist_setup()
     timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
     args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
@@ -266,6 +299,32 @@ def find_actor(args):
     return path_to_actor
 
 
+def push_sweep(args):
+    """The push-recovery grid of `eval --num-envs N --push-speeds ...` as dict(speeds, directions, push_at), or None without push
+    flags; refuses a grid that cannot be run before anything is loaded."""
+    if args.push_speeds is None:
+        if args.push_directions is not None or args.push_at is not None:
+            raise SystemExit("eval --push-directions and --push-at describe the push sweep: add --push-speeds")
+        return None
+    try:
+        speeds = [float(v) for v in args.push_speeds.split(",")]
+    except ValueError:
+        raise SystemExit(f"eval --push-speeds {args.push_speeds!r}: expected comma-separated speeds in m/s, e.g. 0,0.5,1,1.5")
+    if not all(v >= 0 and v < float("inf") for v in speeds):
+        raise SystemExit(f"eval --push-speeds {args.push_speeds}: every speed must be finite and >= 0")
+    directions = 8 if args.push_directions is None else args.push_directions
+    if directions < 1:
+        raise SystemExit(f"eval --push-directions {directions}: needs at least one direction")
+    cells = len(speeds) * directions
+    if args.num_envs < cells:
+        raise SystemExit(f"eval --num-envs {args.num_envs}: the push grid has {len(speeds)} speeds x {directions} directions = {cells} "
+                         "cells, and every cell needs at least one environment")
+    push_at = 2.0 if args.push_at is None else args.push_at
+    if not push_at < float("inf"):
+        raise SystemExit(f"eval --push-at {push_at}: must be a finite number of seconds")
+    return dict(speeds=speeds, directions=directions, push_at=push_at)
+
+
 def evaluate_batched(args):
     """`eval --num-envs N`: the deterministic actor on N environments of the run's env, horizon and YAML, one episode each
     (rl/evaluation.py), with a table of the outcomes and, with --report, the JSON report."""
@@ -273,6 +332,7 @@ def evaluate_batched(args):
         raise SystemExit(f"eval --num-envs {args.num_envs}: needs at least one environment")
     if args.out_dir is not None:
         raise SystemExit("eval --out-dir renders one roll-out to video; it cannot be combined with --num-envs")
+    push = push_sweep(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -280,6 +340,16 @@ def evaluate_batched(args):
     yaml = run_args.yaml
     if yaml is not None and Path(path_to_actor.parent, Path(yaml).name).exists():
         yaml = str(Path(path_to_actor.parent, Path(yaml).name))      # the copy that rode along with the run, as `resume` uses
+    if push is not None:       # the push step needs the run's control step and horizon; refused before the actor is loaded
+        from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
+        from learninghumanoidwalking_b200.model import load_model
+        import_env(run_args.env)
+        mj = load_model(run_args.env)
+        dt = (apply_config(mj, load_yaml(yaml)) if yaml is not None else mj)["cfg"]["control_dt"]
+        k = int(round(push["push_at"] / dt))
+        if not 1 <= k < run_args.max_traj_len:
+            raise SystemExit(f"eval --push-at {push['push_at']}: the push comes after control step {k} of {dt} s, which must lie in "
+                             f"1..{run_args.max_traj_len - 1} (the run's horizon is {run_args.max_traj_len} steps)")
     from learninghumanoidwalking_b200.rl.evaluation import evaluate_batched as run
     from learninghumanoidwalking_b200.rl.policies import install_reference_aliases
     install_reference_aliases()
@@ -288,7 +358,7 @@ def evaluate_batched(args):
     precision = 64 if args.precision is None else args.precision
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
-    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml))
+    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push)
     env.close()
     return report
 
@@ -299,6 +369,8 @@ def evaluate(args):
         return evaluate_batched(args)
     if args.precision is not None or args.report is not None:
         raise SystemExit("eval --precision and --report belong to the batched evaluation: add --num-envs N")
+    if args.push_speeds is not None or args.push_directions is not None or args.push_at is not None:
+        raise SystemExit("eval --push-speeds, --push-directions and --push-at belong to the batched evaluation: add --num-envs N")
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
