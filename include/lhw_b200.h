@@ -112,6 +112,24 @@ int lhw_sim_eval_accumulate(lhw_sim* sim, const void* state_r, const int32_t* st
 int lhw_sim_push(lhw_sim* sim, void* state_r, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
                  const int32_t* ended, double vel, int interval_steps, const void* d, void* stream);
 
+/* lhw_sim_set_command: hold a velocity command (DESIGN.md §7.6; legged_gym's `play` command override, the reference has none).
+ * WalkingTask variants only (jvrc_walk, jvrc_walk_terrain, h1_walk); the others are refused with -2 and a message that names them.
+ * One launch over n envs: an env whose mode [n] (int32) is STANDING = 0, INPLACE = 1 or FORWARD = 2 gets that mode, the held flag
+ * (bit 30 of state_i's mode word, state_i[1]) and mode_ref = ref[i] (ref [n, 3] in the sim's precision, the record's order
+ * (yaw_rate, vx, vy)), and its six task words of obs [n, obs_dim] (from obs_dim - 6: the FORWARD / INPLACE / STANDING one-hot, then
+ * mode_ref) are rewritten as the step would write them.  Any other mode value (-1) leaves the env untouched; nothing else is written.
+ * A held env's step skips the WalkingTask's random mode switches; its next reset (autoreset or lhw_sim_reset) clears the flag.
+ * Reads no model constants. */
+int lhw_sim_set_command(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, const int32_t* mode, const void* ref, void* obs,
+                        void* stream);
+
+/* lhw_sim_command_accumulate: the command sweep's signed velocities of one control step.  After an lhw_sim_step with autoreset == 0
+ * it reads done [n] and the records state_r (only read) and updates acc [n, lhw_sim_command_words()] float64 (zero it before the
+ * first step): while its ended-by-done word is 0, steps, the sums of v_fwd, v_lat and w_z as lhw_sim_eval_accumulate defines
+ * them, and ended-by-done, over exactly the steps that lhw_sim_eval_accumulate counts.  The word layout is sim_core.h's CMD_* enum. */
+int lhw_sim_command_words(void);
+int lhw_sim_command_accumulate(lhw_sim* sim, const void* state_r, int n_envs, const int32_t* done, double* acc, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

@@ -35,6 +35,9 @@ SIGNATURES = {
     "lhw_sim_eval_words": (c_int, []),
     "lhw_sim_eval_accumulate": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 5),
     "lhw_sim_push": (c_int, [c_void_p] * 3 + [c_int, c_uint32, c_uint32, c_void_p, ctypes.c_double, c_int, c_void_p, c_void_p]),
+    "lhw_sim_set_command": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 4),
+    "lhw_sim_command_words": (c_int, []),
+    "lhw_sim_command_accumulate": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 3),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

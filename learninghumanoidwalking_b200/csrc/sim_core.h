@@ -142,6 +142,9 @@ constexpr int MAXPLAN = 128, PLAN_STRIDE = 1 + 3 * NSLAB;   // footstep plan tab
 enum { ST_CURVED = 0, ST_STANDING = 1, ST_BACKWARD = 2, ST_LATERAL = 3, ST_FORWARD = 4 };  // tasks/stepping_task.py:268-271
 
 enum { STANDING = 0, INPLACE = 1, FORWARD = 2 };
+// WalkingTask variants: a mode held by lhw_sim_set_command (DESIGN.md §7.6) carries this bit in the int record's mode word.
+// load_state splits the word into Work::mode and Work::hold and store_state joins them; every other reader masks it off.
+constexpr int32_t MODE_HELD = 1 << 30;
 
 // ---------------------------------------------------------------- math wrappers
 // the transcendental ones are deliberately NOT inlined on the device: each inlined copy of exp/tan/atan2/pow/sincos
@@ -412,6 +415,7 @@ struct alignas(16) Work : Select<Cfg<NJ, TK>::PERENV, PersistRand<real, NJ, TK>,
   real root_vlin[3], foot_vel[2][3], grf[2], cz_min, qacc_lag[3];
   real rew[NREW];
   int iters_total, selfcol, nfloor;   // nfloor: contacts the task's floor-contact queries see (last substep)
+  int hold;   // WalkingTask variants: the mode and reference are held (MODE_HELD); it sits in the tail padding of every variant
 };
 
 // ---------------------------------------------------------------- small vector helpers
@@ -1824,6 +1828,10 @@ LHW_DEV void load_state(Work<real, NJ, TK>& w, const real* sr, const int32_t* si
     for (int it = l; it < NR; it += 32) dst[it] = sr[it];
     if (l == 0) {
       w.phase = si[0]; w.mode = si[1]; w.traj_len = si[2]; w.ep_len = si[3];
+      if constexpr (!Cfg<NJ, TK>::STAND && !Cfg<NJ, TK>::STEP) {
+        w.hold = (si[1] & MODE_HELD) != 0;
+        w.mode = si[1] & ~MODE_HELD;
+      }
       w.rng_ctr = (uint32_t)si[4]; w.have_prev = si[5]; w.status = si[6];
       w.env_id = env_id;
       w.iters_total = 0;
@@ -1839,7 +1847,9 @@ template <class real, int NJ, int TK> LHW_DEV void store_state(const Work<real, 
   LHW_LANES(l) {
     for (int it = l; it < NR; it += 32) sr[it] = src[it];
     if (l == 0) {
-      si[0] = w.phase; si[1] = w.mode; si[2] = w.traj_len; si[3] = w.ep_len;
+      int32_t mode_word = w.mode;
+      if constexpr (!Cfg<NJ, TK>::STAND && !Cfg<NJ, TK>::STEP) mode_word |= w.hold ? MODE_HELD : 0;
+      si[0] = w.phase; si[1] = mode_word; si[2] = w.traj_len; si[3] = w.ep_len;
       si[4] = (int32_t)w.rng_ctr; si[5] = w.have_prev; si[6] = w.status; si[7] = w.iters_total;
     }
   }
@@ -2174,6 +2184,7 @@ template <class real, int NJ, int TK> LHW_DEV void env_reset(Work<real, NJ, TK>&
         philox(seed, w.env_id, w.rng_ctr, 3, u);
         const real c = u01<real>(u[0]);
         w.mode = c < (real)0.6 ? STANDING : (c < (real)0.8 ? INPLACE : FORWARD);
+        w.hold = 0;   // a held command lasts until the env's next reset
         sample_ref<real, NJ, TK>(w, seed, 4);
         w.phase = randint(u[1], m.period);
         if constexpr (Cfg<NJ, TK>::TERRAIN) {
@@ -2263,15 +2274,18 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
       uint32_t u[4];
       philox(seed, w.env_id, w.rng_ctr, 0, u);
       const bool dbl = m.clock[0][w.phase] == (real)1 && m.clock[2][w.phase] == (real)1;
-      if (randint(u[0], 100) == 0 && dbl) {
-        if (w.mode == INPLACE) w.mode = STANDING;
-        else if (w.mode == STANDING) w.mode = INPLACE;
-        sample_ref<real, NJ, TK>(w, seed, 1);
-      }
-      if (randint(u[1], 200) == 0 && w.mode != STANDING) {
-        if (w.mode == FORWARD) w.mode = INPLACE;
-        else if (w.mode == INPLACE) w.mode = FORWARD;
-        sample_ref<real, NJ, TK>(w, seed, 2);
+      // a held command (lhw_sim_set_command) skips both mode switches; the draws are counter-based, so nothing else moves
+      if (!w.hold) {
+        if (randint(u[0], 100) == 0 && dbl) {
+          if (w.mode == INPLACE) w.mode = STANDING;
+          else if (w.mode == STANDING) w.mode = INPLACE;
+          sample_ref<real, NJ, TK>(w, seed, 1);
+        }
+        if (randint(u[1], 200) == 0 && w.mode != STANDING) {
+          if (w.mode == FORWARD) w.mode = INPLACE;
+          else if (w.mode == INPLACE) w.mode = FORWARD;
+          sample_ref<real, NJ, TK>(w, seed, 2);
+        }
       }
       if constexpr (Cfg<NJ, TK>::TERRAIN) {
         if (randint(u[2], m.terrain_interval) == 0 && w.mode != STANDING) terrain_repose<real, NJ, TK>(w, m, seed);
@@ -2474,7 +2488,8 @@ enum { EV_LEN = 0, EV_RET = 1, EV_DONE = 2, EV_TERMS = 3, EV_TRACK = EV_TERMS + 
        EV_WORDS };
 
 // The positions eval_accumulate_env reads in the state record: the persistent block of Work, which load_state / store_state
-// copy in the order Persist [+ PersistStep] declares it, and the int record's mode word (load_state: w.mode = si[1]).
+// copy in the order Persist [+ PersistStep] declares it, and the int record's mode word (load_state: w.mode = si[1] without
+// MODE_HELD).
 template <class real, int NJ, int TK> struct RecordAt {
   static constexpr int NV = 6 + 2 * NJ, NQ = NV + 1, NU = 2 * NJ;
   static constexpr int QPOS = 0, QVEL = NQ, MODE_REF = NQ + 2 * NV + 5 * NU, TK_WORDS = MODE_REF + 4 + 4 * NSLAB;
@@ -2483,6 +2498,19 @@ template <class real, int NJ, int TK> struct RecordAt {
                     sizeof(PersistStep<real, NJ, TK>) == sizeof(real) * (TK_WORDS + 5),
                 "RecordAt must follow the persistent block of Work");
 };
+
+// The root's linear velocity in its own frame, (R^T v)[0:2] with v = qvel[0:3] (world) and R the rotation of the quaternion
+// qpos[3:7] (normalised in the formula): v_fwd and v_lat of DESIGN.md §7.4, in float64 at either precision.
+template <class real, int NJ, int TK> LHW_DEV void root_frame_velocity(const real* sr, double& vf, double& vl) {
+  using A = RecordAt<real, NJ, TK>;
+  const double qw = (double)sr[A::QPOS + 3], x = (double)sr[A::QPOS + 4], y = (double)sr[A::QPOS + 5], z = (double)sr[A::QPOS + 6];
+  const double s = 2 / (qw * qw + x * x + y * y + z * z);
+  const double X = x * s, Y = y * s, Z = z * s;
+  const double wX = qw * X, wY = qw * Y, wZ = qw * Z, xX = x * X, xY = x * Y, xZ = x * Z, yY = y * Y, yZ = y * Z, zZ = z * Z;
+  const double v0 = (double)sr[A::QVEL + 0], v1 = (double)sr[A::QVEL + 1], v2 = (double)sr[A::QVEL + 2];
+  vf = (1 - (yY + zZ)) * v0 + (xY + wZ) * v1 + (xZ - wY) * v2;   // (R^T v)[0]
+  vl = (xY - wZ) * v0 + (1 - (xX + zZ)) * v1 + (yZ + wX) * v2;   // (R^T v)[1]
+}
 
 // One control step of one env into its accumulator acc[EV_WORDS], from the step's outputs (reward, rew_terms[NREW], done) and
 // the record it left (autoreset off).  An env counts the steps up to and including the first with done set; after that its
@@ -2499,18 +2527,14 @@ LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward,
     acc[EV_REACHED] = (double)sr[A::TK_WORDS + 1];
     acc[EV_SEQLEN] = (double)sr[A::TK_WORDS + 0];
   } else {
-    const int mode = Cfg<NJ, TK>::STAND ? (int)STANDING : si[A::I_MODE];   // the StandingTask holds zero references
+    // the StandingTask holds zero references; a held WalkingTask mode carries MODE_HELD
+    const int mode = Cfg<NJ, TK>::STAND ? (int)STANDING : si[A::I_MODE] & ~MODE_HELD;
     double yaw_ref = (double)sr[A::MODE_REF + 0], vx = (double)sr[A::MODE_REF + 1], vy = (double)sr[A::MODE_REF + 2];
     if (mode == STANDING) { yaw_ref = vx = vy = 0; }
     else if (mode == INPLACE) { vx = vy = 0; }
     else { yaw_ref = 0; }
-    const double qw = (double)sr[A::QPOS + 3], x = (double)sr[A::QPOS + 4], y = (double)sr[A::QPOS + 5], z = (double)sr[A::QPOS + 6];
-    const double s = 2 / (qw * qw + x * x + y * y + z * z);
-    const double X = x * s, Y = y * s, Z = z * s;
-    const double wX = qw * X, wY = qw * Y, wZ = qw * Z, xX = x * X, xY = x * Y, xZ = x * Z, yY = y * Y, yZ = y * Z, zZ = z * Z;
-    const double v0 = (double)sr[A::QVEL + 0], v1 = (double)sr[A::QVEL + 1], v2 = (double)sr[A::QVEL + 2];
-    const double vf = (1 - (yY + zZ)) * v0 + (xY + wZ) * v1 + (xZ - wY) * v2;   // (R^T v)[0]
-    const double vl = (xY - wZ) * v0 + (1 - (xX + zZ)) * v1 + (yZ + wX) * v2;   // (R^T v)[1]
+    double vf, vl;
+    root_frame_velocity<real, NJ, TK>(sr, vf, vl);
     double* t = acc + EV_TRACK + 4 * mode;
     t[0] += 1;
     t[1] += m_abs(vf - vx);
@@ -2559,6 +2583,41 @@ LHW_DEV int push_env(real* sr, const int32_t* si, uint32_t seed, uint32_t env_id
   sr[A::QVEL + 0] = (real)((double)sr[A::QVEL + 0] + (c * dx - s * dy));
   sr[A::QVEL + 1] = (real)((double)sr[A::QVEL + 1] + (s * dx + c * dy));
   return 1;
+}
+
+// ================================================================= held commands (lhw_sim_set_command, DESIGN.md §7.6)
+// legged_gym's `play` command override for the WalkingTask variants.  A command sets the env's mode and reference and holds them:
+// the step skips its two random mode switches while MODE_HELD is set, and env_reset clears it.  The body writes the mode word,
+// mode_ref and the six task words of the observation (the FORWARD / INPLACE / STANDING one-hot, then mode_ref, as env_obs writes
+// them), so the next action already sees the command; nothing else, and nothing of an env whose mode is not 0..2 (-1: untouched).
+// ref = (yaw_rate, vx, vy), the record's order.  Returns 1 when the env was given the command.
+template <class real, int NJ, int TK>
+LHW_DEV int set_command_env(real* sr, int32_t* si, int32_t mode, const real* ref, real* obs) {
+  static_assert(!Cfg<NJ, TK>::STAND && !Cfg<NJ, TK>::STEP, "only the WalkingTask variants take a velocity command");
+  using A = RecordAt<real, NJ, TK>;
+  if (mode < STANDING || mode > FORWARD) return 0;
+  si[A::I_MODE] = mode | MODE_HELD;
+  real* e = obs + Dims<real, NJ, TK>::NROBOT + 2;
+  e[0] = mode == FORWARD; e[1] = mode == INPLACE; e[2] = mode == STANDING;
+  for (int x = 0; x < 3; x++) sr[A::MODE_REF + x] = e[3 + x] = ref[x];
+  return 1;
+}
+
+// The command sweep's signed velocities (lhw_sim_command_accumulate): per env, float64 words [steps, sum v_fwd, sum v_lat,
+// sum w_z, ended-by-done], with v_fwd, v_lat and w_z as eval_accumulate_env defines them, over the same steps: up to and including
+// the first with done set.
+enum { CMD_LEN = 0, CMD_VF = 1, CMD_VL = 2, CMD_WZ = 3, CMD_DONE = 4, CMD_WORDS };
+
+template <class real, int NJ, int TK> LHW_DEV void command_accumulate_env(const real* sr, int32_t done, double* acc) {
+  using A = RecordAt<real, NJ, TK>;
+  if (acc[CMD_DONE] != 0) return;
+  double vf, vl;
+  root_frame_velocity<real, NJ, TK>(sr, vf, vl);
+  acc[CMD_LEN] += 1;
+  acc[CMD_VF] += vf;
+  acc[CMD_VL] += vl;
+  acc[CMD_WZ] += (double)sr[A::QVEL + 5];
+  if (done) acc[CMD_DONE] = 1;
 }
 
 }  // namespace lhw

@@ -196,6 +196,27 @@ __global__ void __launch_bounds__(256) push_kernel(real* __restrict__ state_r, c
                          ended ? ended[env] : 0, vel, interval, d ? d + 2 * (size_t)env : nullptr);
 }
 
+// held commands (WalkingTask variants only): one thread per env, the mode word, mode_ref and the obs task words of the envs given
+// one (sim_core.h set_command_env)
+template <class real, int NJ, int TK>
+__global__ void __launch_bounds__(256) set_command_kernel(real* __restrict__ state_r, int32_t* __restrict__ state_i, int n_envs,
+                                                         const int32_t* __restrict__ mode, const real* __restrict__ ref,
+                                                         real* __restrict__ obs) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= n_envs) return;
+  set_command_env<real, NJ, TK>(state_r + (size_t)env * Dims<real, NJ, TK>::NSTATE_R, state_i + (size_t)env * NSTATE_I, mode[env],
+                                ref + 3 * (size_t)env, obs + (size_t)env * Dims<real, NJ, TK>::NOBS);
+}
+
+// the command sweep's signed velocities: one thread per env, the record only read (sim_core.h command_accumulate_env)
+template <class real, int NJ, int TK>
+__global__ void __launch_bounds__(256) command_accumulate_kernel(const real* __restrict__ state_r, int n_envs,
+                                                                const int32_t* __restrict__ done, double* __restrict__ acc) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= n_envs) return;
+  command_accumulate_env<real, NJ, TK>(state_r + (size_t)env * Dims<real, NJ, TK>::NSTATE_R, done[env], acc + (size_t)env * CMD_WORDS);
+}
+
 }  // namespace
 
 // what every sim has, whichever its variant; SimOf<real, NJ, TK> holds its model and launches its kernels
@@ -216,6 +237,9 @@ struct lhw_sim {
                                const int32_t* done, double* acc, cudaStream_t st) = 0;
   virtual void push(void* state_r, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* ended,
                     double vel, int interval, const void* d, cudaStream_t st) = 0;
+  virtual int set_command(void* state_r, int32_t* state_i, int n_envs, const int32_t* mode, const void* ref, void* obs,
+                          cudaStream_t st) = 0;
+  virtual void command_accumulate(const void* state_r, int n_envs, const int32_t* done, double* acc, cudaStream_t st) = 0;
   virtual void set_step_height(double h) = 0;
 };
 
@@ -333,6 +357,22 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
             int interval, const void* d, cudaStream_t st) override {
     push_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, ended, vel,
                                                                     interval, (const real*)d);
+  }
+
+  int set_command(void* state_r, int32_t* state_i, int n_envs, const int32_t* mode, const void* ref, void* obs,
+                  cudaStream_t st) override {
+    if constexpr (Cfg<NJ, TK>::STAND || Cfg<NJ, TK>::STEP) {
+      return fail(-2, std::string(Cfg<NJ, TK>::STEP ? "jvrc_step (SteppingTask)" : "h1 (StandingTask)") +
+                          " has no velocity command: only the WalkingTask variants jvrc_walk, jvrc_walk_terrain and h1_walk take one");
+    } else {
+      set_command_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((real*)state_r, state_i, n_envs, mode, (const real*)ref,
+                                                                             (real*)obs);
+      return 0;
+    }
+  }
+
+  void command_accumulate(const void* state_r, int n_envs, const int32_t* done, double* acc, cudaStream_t st) override {
+    command_accumulate_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((const real*)state_r, n_envs, done, acc);
   }
 
   void set_step_height(double h) override {
@@ -459,6 +499,28 @@ int lhw_sim_push(lhw_sim* s, void* state_r, const int32_t* state_i, int n_envs, 
   if (!d && interval_steps < 1) return fail(-2, "push interval must be at least one control step");
   if (n_envs <= 0) return 0;
   s->push(state_r, state_i, n_envs, seed, first_env_id, ended, vel, interval_steps, d, (cudaStream_t)stream);   // no model constants
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_set_command(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, const int32_t* mode, const void* ref, void* obs,
+                        void* stream) {
+  if (!s || !state_r || !state_i || !mode || !ref || !obs) return fail(-1, "null argument");
+  if (n_envs <= 0) return 0;
+  const int rc = s->set_command(state_r, state_i, n_envs, mode, ref, obs, (cudaStream_t)stream);   // no model constants
+  if (rc) return rc;
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_command_words(void) { return CMD_WORDS; }
+
+int lhw_sim_command_accumulate(lhw_sim* s, const void* state_r, int n_envs, const int32_t* done, double* acc, void* stream) {
+  if (!s || !state_r || !done || !acc) return fail(-1, "null argument");
+  if (n_envs <= 0) return 0;
+  s->command_accumulate(state_r, n_envs, done, acc, (cudaStream_t)stream);   // reads no model constants
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -141,6 +141,35 @@ void sim_push(int64_t sim, Tensor state_r, const Tensor& state_i, int64_t seed, 
   ok(lhw_sim_push(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
                   ended ? ended->data_ptr<int32_t>() : nullptr, vel, (int)interval_steps, d ? d->data_ptr() : nullptr, stream_of(state_r)),
      "lhw_sim_push");
+}
+
+void sim_set_command(int64_t sim, Tensor state_r, Tensor state_i, const Tensor& mode, const Tensor& ref, Tensor obs) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  check_cuda(mode, "mode", at::kInt, I.device); check_shape(mode, "mode", {n});
+  check_cuda(ref, "ref", I.real, I.device); check_shape(ref, "ref", {n, 3});
+  check_cuda(obs, "obs", I.real, I.device); check_shape(obs, "obs", {n, I.nobs});
+  c10::cuda::CUDAGuard guard(I.device);
+  // called once per episode, outside graphs: the host syncs on the values are affordable
+  TORCH_CHECK(!((mode < -1) | (mode > 2)).any().item<bool>(), "lhw: mode must be -1 (untouched), 0 (STANDING), 1 (INPLACE) or 2 (FORWARD)");
+  TORCH_CHECK(ref.isfinite().all().item<bool>(), "lhw: ref must be finite");
+  ok(lhw_sim_set_command(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, mode.data_ptr<int32_t>(), ref.data_ptr(),
+                         obs.data_ptr(), stream_of(state_r)), "lhw_sim_set_command");
+}
+
+void sim_command_accumulate(int64_t sim, const Tensor& state_r, const Tensor& done, Tensor acc) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
+  check_cuda(done, "done", at::kInt, I.device); check_shape(done, "done", {n});
+  check_cuda(acc, "acc", at::kDouble, I.device); check_shape(acc, "acc", {n, lhw_sim_command_words()});
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_command_accumulate(I.s, state_r.data_ptr(), (int)n, done.data_ptr<int32_t>(), acc.data_ptr<double>(), stream_of(state_r)),
+     "lhw_sim_command_accumulate");
 }
 
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
@@ -346,6 +375,8 @@ TORCH_LIBRARY(lhw, m) {
   m.def("sim_eval_accumulate(int sim, Tensor state_r, Tensor state_i, Tensor reward, Tensor rew_terms, Tensor done, Tensor(a!) acc) -> ()");
   m.def("sim_push(int sim, Tensor(a!) state_r, Tensor state_i, int seed, int first_env_id, Tensor? ended, float vel, int interval_steps, "
         "Tensor? d) -> ()");
+  m.def("sim_set_command(int sim, Tensor(a!) state_r, Tensor(b!) state_i, Tensor mode, Tensor ref, Tensor(c!) obs) -> ()");
+  m.def("sim_command_accumulate(int sim, Tensor state_r, Tensor done, Tensor(a!) acc) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -377,6 +408,8 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_render", &sim_render);
   m.impl("sim_eval_accumulate", &sim_eval_accumulate);
   m.impl("sim_push", &sim_push);
+  m.impl("sim_set_command", &sim_set_command);
+  m.impl("sim_command_accumulate", &sim_command_accumulate);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

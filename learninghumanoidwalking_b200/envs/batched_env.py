@@ -24,6 +24,10 @@ STAND_REWARD_NAMES = ("com_vel_error", "yaw_vel_error", "height", "upperbody", "
                       "posture")                                                          # tasks/standing_task.py:97-104
 STEP_REWARD_NAMES = ("foot_frc_score", "foot_vel_score", "orient_cost", "height_error", "step_reward",
                      "upper_body_reward")                                                 # tasks/stepping_task.py:107-120
+# held velocity commands (set_command, DESIGN.md §7.6): the WalkingTask envs, and the held flag of the kernel's mode word
+# (csrc/sim_core.h MODE_HELD)
+COMMAND_ENVS = ("jvrc_walk", "jvrc_walk_terrain", "h1_walk")
+MODE_HELD = 1 << 30
 N_REWARD_SLOTS = 10   # width of the kernel's reward-term record (csrc/sim_core.h NREW); unused slots are 0
 # h1_walk (DESIGN.md §4.6): joints (hip_yaw, hip_roll, hip_pitch, knee, ankle), left leg then right.  The mirror swaps the legs and
 # negates yaw and roll; in the observation also the root roll and the x, z angular velocities.  The 8 walking-task words map to
@@ -245,6 +249,38 @@ class BatchedHumanoidEnv:
         if d.dtype != self.dtype or not d.is_contiguous() or d.device != self.device:
             d = d.to(device=self.device, dtype=self.dtype).contiguous()
         _lib.ops().sim_push(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, None, 0.0, 1, d)
+
+    def set_command(self, mode, ref) -> None:
+        """Give environments a velocity command and hold it until each one's next reset: mode [N] holds per env -1 (untouched),
+        0 (STANDING), 1 (INPLACE) or 2 (FORWARD), and ref [N, 3] its reference (yaw_rate rad/s, vx m/s, vy m/s), in the order of the
+        record's mode_ref; sequences or tensors.  The WalkingTask's random mode switches skip a held env, and the six task words of
+        self.obs are rewritten, so the next action already sees the command (include/lhw_b200.h: lhw_sim_set_command).  Values
+        outside the training ranges (DESIGN.md §7.6) are accepted; non-finite ones and other modes are refused."""
+        if self.model_name not in COMMAND_ENVS:
+            raise ValueError(f"{self.model_name} has no velocity command: only the WalkingTask envs {', '.join(COMMAND_ENVS)} take one")
+        mode = torch.as_tensor(mode).detach().to("cpu").reshape(-1)
+        ref = torch.as_tensor(ref, dtype=torch.float64).detach().to("cpu")
+        if mode.dtype.is_floating_point or mode.dtype == torch.bool or mode.shape != (self.num_envs,):
+            raise ValueError(f"mode must hold {self.num_envs} integers, got {tuple(mode.shape)} of {mode.dtype}")
+        if ref.shape != (self.num_envs, 3):
+            raise ValueError(f"ref must be [{self.num_envs}, 3] (yaw_rate, vx, vy), got {tuple(ref.shape)}")
+        if ((mode < -1) | (mode > 2)).any():
+            raise ValueError(f"mode must be -1 (untouched), 0 (STANDING), 1 (INPLACE) or 2 (FORWARD), got {sorted(set(mode.tolist()))}")
+        if not torch.isfinite(ref).all():
+            raise ValueError("ref must be finite")
+        _lib.ops().sim_set_command(self._h.value, self.state_r, self.state_i, mode.to(device=self.device, dtype=torch.int32),
+                                   ref.to(device=self.device, dtype=self.dtype), self.obs)
+
+    def command_accumulate(self, acc: torch.Tensor) -> torch.Tensor:
+        """Add the last control step (taken with autoreset=False) to the command sweep's signed-velocity records acc, a
+        zero-initialised [N, command_words()] float64 device tensor: steps, the sums of v_fwd, v_lat and w_z, ended-by-done, over
+        the steps eval_accumulate counts (include/lhw_b200.h: lhw_sim_command_accumulate)."""
+        _lib.ops().sim_command_accumulate(self._h.value, self.state_r, self.done, acc)
+        return acc
+
+    @staticmethod
+    def command_words() -> int:
+        return _lib.lib().lhw_sim_command_words()
 
     def eval_accumulate(self, acc: torch.Tensor) -> torch.Tensor:
         """Add the last control step (taken with autoreset=False) to the evaluation accumulators acc, a zero-initialised

@@ -10,6 +10,10 @@ The push-recovery sweep (`eval --num-envs N --push-speeds ...`, DESIGN.md §7.5)
 K = round(push_at / dt), between two replays of the same graph: env i gets the speed and heading-frame direction of grid cell
 i mod (speeds x directions).  A fallen env is not pushed (a device-side `where` on its ended-by-done word), and the statistics come
 from the same accumulator words: fell before the push (EV_DONE set and EV_LEN <= K), survived (EV_DONE clear at the horizon).
+
+The command-tracking sweep (`eval --num-envs N --command forward:0,0.2 inplace:0.4 standing`, DESIGN.md §7.6) gives env i the held
+command of cell i mod C (BatchedHumanoidEnv.set_command) after the reset, before the first step and outside the graph.  The graph
+body then also launches BatchedHumanoidEnv.command_accumulate, whose per-env records give the signed mean velocities of each cell.
 """
 from __future__ import annotations
 
@@ -22,6 +26,8 @@ import torch
 LEN, RET, DONE, TERMS, TRACK, REACHED, SEQLEN, WORDS = 0, 1, 2, 3, 13, 25, 26, 27
 MODES = ("STANDING", "INPLACE", "FORWARD")     # WalkingTask's modes, in the order of the kernel's mode word
 TRACKED = ("jvrc_walk", "jvrc_walk_terrain", "h1_walk", "h1")   # h1: its StandingTask, against zero references
+# the command sweep's signed-velocity words of csrc/sim_core.h (CMD_*), per env
+C_LEN, C_VF, C_VL, C_WZ, C_DONE, C_WORDS = 0, 1, 2, 3, 4, 5
 
 
 def push_grid(n: int, speeds, directions: int):
@@ -37,16 +43,39 @@ def push_vectors(speed: np.ndarray, dir_deg: np.ndarray) -> np.ndarray:
     return np.stack((speed * np.cos(th), speed * np.sin(th)), axis=1)
 
 
+def command_grid(n: int, cells):
+    """Per env (mode index, value) of the command sweep: env i is in cell i mod C of cells = [(mode name, value), ...]."""
+    c = np.arange(n) % len(cells)
+    return np.asarray([MODES.index(m) for m, _ in cells], dtype=np.int32)[c], np.asarray([v for _, v in cells], dtype=np.float64)[c]
+
+
+def command_refs(mode: np.ndarray, value: np.ndarray) -> np.ndarray:
+    """[N, 3] references (yaw_rate, vx, vy) of the sweep: FORWARD value -> (0, value, 0), INPLACE value -> (value, 0, 0), STANDING
+    -> (0, 0, 0)."""
+    ref = np.zeros((len(mode), 3))
+    ref[mode == MODES.index("FORWARD"), 1] = value[mode == MODES.index("FORWARD")]
+    ref[mode == MODES.index("INPLACE"), 0] = value[mode == MODES.index("INPLACE")]
+    return ref
+
+
 @torch.no_grad()
-def rollout(env, policy, steps: int, graph: bool = True, push=None) -> torch.Tensor:
+def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None):
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
     [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
     push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
-    change d [N, 2] (BatchedHumanoidEnv.push); with push=None nothing but the control steps is launched."""
+    change d [N, 2] (BatchedHumanoidEnv.push); with push=None nothing but the control steps is launched.
+    command = (mode [N], ref [N, 3]): held commands (BatchedHumanoidEnv.set_command) applied after the reset, and every step also
+    adds to the [N, C_WORDS] signed-velocity records; then the return is (accumulators, signed-velocity records)."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
+    if command is not None and env.command_words() != C_WORDS:
+        raise RuntimeError(f"the library's command record has {env.command_words()} words, this module knows {C_WORDS}")
     acc = torch.zeros(env.num_envs, WORDS, dtype=torch.float64, device=env.device)
-    state = env.reset().float().clone()
+    cacc = torch.zeros(env.num_envs, C_WORDS, dtype=torch.float64, device=env.device) if command is not None else None
+    env.reset()
+    if command is not None:
+        env.set_command(*command)
+    state = env.obs.float().clone()
     push_k, push_d = push if push is not None else (None, None)
     if push is not None:
         if not 1 <= push_k < steps:
@@ -61,13 +90,16 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None) -> torch.Ten
         a = policy(state, deterministic=True)
         obs, _, _, _ = env.step(a if env.dtype == torch.float32 else a.double(), autoreset=False)
         env.eval_accumulate(acc)
+        if cacc is not None:
+            env.command_accumulate(cacc)
         state.copy_(obs.float())
 
+    out = acc if command is None else (acc, cacc)
     if not graph or steps <= 1:
         for t in range(steps):
             body()
             after(t + 1)
-        return acc
+        return out
     cur = torch.cuda.current_stream(env.device)
     s = torch.cuda.Stream(device=env.device)
     s.wait_stream(cur)
@@ -82,7 +114,7 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None) -> torch.Ten
             g.replay()
             after(t)
     cur.wait_stream(s)
-    return acc
+    return out
 
 
 def summarize(acc: np.ndarray, env_name: str, reward_names) -> dict:
@@ -160,6 +192,38 @@ def format_push_table(p: dict) -> str:
     return "\n".join(lines)
 
 
+def command_summary(acc: np.ndarray, cacc: np.ndarray, mode: np.ndarray, value: np.ndarray, cells) -> dict:
+    """The command sweep's outcome per cell: n, fall fraction, mean episode length; the achieved v_fwd, v_lat and w_z as the mean
+    and standard deviation over the cell's envs of each env's per-step mean; and the §7.4 tracking errors of the held mode, the
+    cell's error sums over its tracked steps."""
+    v = cacc[:, [C_VF, C_VL, C_WZ]] / cacc[:, C_LEN:C_LEN + 1]
+    out = []
+    for name, val in cells:
+        m_idx = MODES.index(name)
+        m = (mode == m_idx) & (value == float(val))
+        ref = command_refs(np.array([m_idx]), np.array([float(val)]))[0]
+        t = acc[m, TRACK + 4 * m_idx:TRACK + 4 * m_idx + 4].sum(0)
+        achieved = {k: dict(mean=float(v[m, j].mean()), std=float(v[m, j].std())) for j, k in enumerate(("v_fwd", "v_lat", "yaw_rate"))}
+        out.append(dict(mode=name, value=float(val), ref=dict(yaw_rate=float(ref[0]), vx=float(ref[1]), vy=float(ref[2])), n=int(m.sum()),
+                        fall_fraction=float((acc[m, DONE] != 0).mean()), mean_length=float(acc[m, LEN].mean()), achieved=achieved,
+                        tracking=dict(steps=int(t[0]), vx_error=float(t[1] / t[0]), vy_error=float(t[2] / t[0]),
+                                      yaw_rate_error=float(t[3] / t[0]))))
+    return dict(cells=out)
+
+
+def format_command_table(c: dict) -> str:
+    f = lambda a: f"{a['mean']:>7.3f} +- {a['std']:.3f}"
+    lines = ["  held commands: achieved = mean over the cell's envs of each env's per-step mean (+- std across envs)",
+             "    command              n   fell  length        v_fwd m/s         v_lat m/s         w_z rad/s"
+             "   |v_fwd-vx| |v_lat-vy| |w_z-yaw|"]
+    for x in c["cells"]:
+        a, t = x["achieved"], x["tracking"]
+        name = x["mode"].lower() + ("" if x["mode"] == "STANDING" else f" {x['value']:g}")
+        lines.append(f"    {name:<16s} {x['n']:>5d} {x['fall_fraction']:6.3f} {x['mean_length']:7.1f}  {f(a['v_fwd'])}  {f(a['v_lat'])}  "
+                     f"{f(a['yaw_rate'])}  {t['vx_error']:10.4f} {t['vy_error']:10.4f} {t['yaw_rate_error']:9.4f}")
+    return "\n".join(lines)
+
+
 def format_table(s: dict, max_traj_len: int) -> str:
     L = s["length"]
     lines = [f"{s['num_envs']} environments, one episode each, horizon {max_traj_len} control steps",
@@ -180,16 +244,23 @@ def format_table(s: dict, max_traj_len: int) -> str:
     return "\n".join(lines)
 
 
-def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None) -> dict:
+def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
     out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
-    push-recovery sweep, with its table and `summary.push`.  Returns the report."""
-    sweep = None
+    push-recovery sweep, with its table and `summary.push`.  commands = [(mode name, value), ...]: the command-tracking sweep
+    (env i holds the command of cell i mod len(commands)), with its table and `summary.commands`.  Returns the report."""
+    if push is not None and commands is not None:
+        raise ValueError("the push sweep and the command sweep are separate evaluations")
+    sweep = held = None
     if push is not None:
         k = int(round(push["push_at"] / env.dt))
         speed, dir_deg = push_grid(env.num_envs, push["speeds"], push["directions"])
         sweep = (k, push_vectors(speed, dir_deg))
-    acc = rollout(env, policy, env.max_traj_len, push=sweep).cpu().numpy()
+    if commands is not None:
+        cmd_mode, cmd_value = command_grid(env.num_envs, commands)
+        held = (cmd_mode, command_refs(cmd_mode, cmd_value))
+    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held)
+    acc, cacc = (out[0].cpu().numpy(), out[1].cpu().numpy()) if commands is not None else (out.cpu().numpy(), None)
     summary = summarize(acc, env.model_name, env.reward_names)
     pe = per_env(acc, env.model_name, env.reward_names)
     print(format_table(summary, env.max_traj_len))
@@ -197,6 +268,12 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         summary["push"] = push_summary(acc, speed, dir_deg, push["speeds"], push["directions"], push["push_at"], k)
         pe.update(push_speed=speed.tolist(), push_dir_deg=dir_deg.tolist())
         print(format_push_table(summary["push"]))
+    if commands is not None:
+        summary["commands"] = command_summary(acc, cacc, cmd_mode, cmd_value, commands)
+        pe.update(command_mode=[MODES[m] for m in cmd_mode], command_value=cmd_value.tolist(),
+                  command_steps=cacc[:, C_LEN].astype(int).tolist(), v_fwd_sum=cacc[:, C_VF].tolist(),
+                  v_lat_sum=cacc[:, C_VL].tolist(), yaw_rate_sum=cacc[:, C_WZ].tolist())
+        print(format_command_table(summary["commands"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
                   max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:

@@ -56,7 +56,8 @@ class _DeviceTask(BaseTask):
 
     @property
     def mode(self) -> int:
-        return int(self._env.state_i[self._index, 1].item())
+        from ..envs.batched_env import MODE_HELD
+        return int(self._env.state_i[self._index, 1].item()) & ~MODE_HELD   # without the held-command flag
 
 
 class WalkingTask(_DeviceTask):

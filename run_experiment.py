@@ -22,7 +22,10 @@ KL after every minibatch (rsl_rl's schedule, DESIGN §7.3); the rate is printed 
 evaluation batches run on the training env and see the pushes too; `resume` rebuilds the env with the run's values, and a run
 recorded without them has none.  `eval --num-envs N --push-speeds 0,0.5,1,1.5 [--push-directions 8] [--push-at 2.0]` pushes each
 env once, at --push-at seconds, with the speed and direction of its cell of the grid (env i: cell i mod speeds x directions), and
-prints the survival of each cell; the batched evaluation never gets the training pushes.
+prints the survival of each cell; the batched evaluation never gets the training pushes.  `eval --command forward:0,0.2,0.4
+inplace:-0.4,0.4 standing` holds walking commands (DESIGN §7.6): with --num-envs N env i holds the command of cell i mod C and the
+run prints the achieved velocities and tracking errors of each cell; without it, the one command is held on the single-env roll-out
+(and its video) and re-applied after every reset there.
 """
 import argparse
 import os
@@ -81,7 +84,11 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
               # push-recovery sweep of the batched evaluation (DESIGN §7.5)
               ("--push-speeds", dict(type=_S, default=None, help="with --num-envs: comma-separated push speeds in m/s, e.g. 0,0.5,1,1.5")),
               ("--push-directions", dict(type=_I, default=None, help="push directions, evenly spaced from forward (default 8)")),
-              ("--push-at", dict(type=_F, default=None, help="seconds into the episode of the one push (default 2.0)"))]
+              ("--push-at", dict(type=_F, default=None, help="seconds into the episode of the one push (default 2.0)")),
+              # held walking commands (DESIGN §7.6)
+              ("--command", dict(type=_S, nargs="+", action="extend", default=None,
+                                 help="held walking commands MODE[:v1,v2,...]: forward:V m/s, inplace:W rad/s, standing; with "
+                                      "--num-envs one cell per (mode, value), else exactly one"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -325,6 +332,50 @@ def push_sweep(args):
     return dict(speeds=speeds, directions=directions, push_at=push_at)
 
 
+COMMAND_MODES = {"forward": "FORWARD", "inplace": "INPLACE", "standing": "STANDING"}
+
+
+def command_cells(args):
+    """The held commands of `eval --command ...` as [(mode name, value), ...] (rl/evaluation.py MODES), or None without the flag;
+    refuses a list that cannot be run before anything is loaded.  Values outside the training ranges are allowed."""
+    if args.command is None:
+        return None
+    cells = []
+    for spec in args.command:
+        name, sep, values = spec.partition(":")
+        if name not in COMMAND_MODES:
+            raise SystemExit(f"eval --command {spec!r}: unknown mode {name!r}; expected forward:V[,V...], inplace:W[,W...] or standing")
+        if name == "standing":
+            if sep:
+                raise SystemExit(f"eval --command {spec!r}: standing takes no values")
+            cells.append(("STANDING", 0.0))
+            continue
+        try:
+            vs = [float(v) for v in values.split(",")]
+        except ValueError:
+            raise SystemExit(f"eval --command {spec!r}: expected {name}:V[,V...] with comma-separated numbers "
+                             f"({'m/s' if name == 'forward' else 'rad/s'})")
+        if not all(abs(v) < float("inf") for v in vs):
+            raise SystemExit(f"eval --command {spec!r}: every value must be finite")
+        cells += [(COMMAND_MODES[name], v) for v in vs]
+    if args.push_speeds is not None:
+        raise SystemExit("eval --command and --push-speeds are separate sweeps: run them one at a time")
+    if args.num_envs is None and len(cells) > 1:
+        raise SystemExit(f"eval --command: {len(cells)} commands need the batched evaluation (add --num-envs N); the single-env "
+                         "roll-out holds exactly one")
+    if args.num_envs is not None and args.num_envs < len(cells):
+        raise SystemExit(f"eval --num-envs {args.num_envs}: --command lists {len(cells)} cells, and every cell needs at least one "
+                         "environment")
+    return cells
+
+
+def check_command_env(env_name):
+    """Refuse --command for a run whose env has no walking command, before its actor is loaded."""
+    from learninghumanoidwalking_b200.envs.batched_env import COMMAND_ENVS
+    if env_name not in COMMAND_ENVS:
+        raise SystemExit(f"eval --command: the run's env {env_name} has no walking command; only {', '.join(COMMAND_ENVS)} take one")
+
+
 def evaluate_batched(args):
     """`eval --num-envs N`: the deterministic actor on N environments of the run's env, horizon and YAML, one episode each
     (rl/evaluation.py), with a table of the outcomes and, with --report, the JSON report."""
@@ -333,10 +384,13 @@ def evaluate_batched(args):
     if args.out_dir is not None:
         raise SystemExit("eval --out-dir renders one roll-out to video; it cannot be combined with --num-envs")
     push = push_sweep(args)
+    commands = command_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
         run_args = pickle.load(f)
+    if commands is not None:
+        check_command_env(run_args.env)
     yaml = run_args.yaml
     if yaml is not None and Path(path_to_actor.parent, Path(yaml).name).exists():
         yaml = str(Path(path_to_actor.parent, Path(yaml).name))      # the copy that rode along with the run, as `resume` uses
@@ -358,7 +412,7 @@ def evaluate_batched(args):
     precision = 64 if args.precision is None else args.precision
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
-    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push)
+    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands)
     env.close()
     return report
 
@@ -371,10 +425,13 @@ def evaluate(args):
         raise SystemExit("eval --precision and --report belong to the batched evaluation: add --num-envs N")
     if args.push_speeds is not None or args.push_directions is not None or args.push_at is not None:
         raise SystemExit("eval --push-speeds, --push-directions and --push-at belong to the batched evaluation: add --num-envs N")
+    commands = command_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
         run_args = pickle.load(f)
+    if commands is not None:
+        check_command_env(run_args.env)
     cv2 = None
     if args.out_dir is not None:
         try:
@@ -387,7 +444,16 @@ def evaluate(args):
     policy = torch.load(path_to_actor, weights_only=False).cuda().eval()
     print_system_info(args, training=False)
     env = import_env(run_args.env)(1, precision=64, seed=args.seed or 0)
-    obs = env.reset().float()
+
+    def reset():
+        env.reset()
+        if commands is not None:     # the one command, held again after every reset
+            from learninghumanoidwalking_b200.rl.evaluation import command_grid, command_refs
+            mode, value = command_grid(1, commands)
+            env.set_command(mode, command_refs(mode, value))
+        return env.obs.float()
+
+    obs = reset()
     n_steps = int(args.ep_len / env.dt)
     video = None
     if cv2 is not None:
@@ -412,7 +478,7 @@ def evaluate(args):
             if bool(done[0]):
                 episodes.append((ep_len, ep_ret))
                 ep_ret, ep_len = 0.0, 0
-                obs = env.reset()
+                obs = reset()
             obs = obs.float()
     episodes.append((ep_len, ep_ret))
     print(f"{len(episodes)} episode(s) in {n_steps} control steps: " + ", ".join(f"len {l} return {r:.2f}" for l, r in episodes))
