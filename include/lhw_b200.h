@@ -130,6 +130,18 @@ int lhw_sim_set_command(lhw_sim* sim, void* state_r, int32_t* state_i, int n_env
 int lhw_sim_command_words(void);
 int lhw_sim_command_accumulate(lhw_sim* sim, const void* state_r, int n_envs, const int32_t* done, double* acc, void* stream);
 
+/* lhw_sim_reset_footsteps: lhw_sim_reset with a chosen stepping-stone plan (DESIGN.md §7.7).  jvrc_step only; the other variants
+ * are refused with -2 and a message that names them.  An env whose mode [n] (int32) is an ST_* value (CURVED = 0, STANDING = 1,
+ * BACKWARD = 2, LATERAL = 3, FORWARD = 4) is reset as lhw_sim_reset resets it, with that plan type and value [n] (the sim's
+ * precision): FORWARD the signed stair height in m (for the sign draw and the curriculum height), LATERAL the side +1 (the robot's
+ * left) or -1, CURVED a plan index in [0, nplan) (any other value: the reset's own draw), STANDING and BACKWARD 0.  Every other
+ * draw is the plain reset's.  Any other mode (-1) leaves the env untouched.  `fresh` and obs as for lhw_sim_reset.  The plan
+ * lasts for the episode: the next reset draws one again.
+ * lhw_sim_footstep_limits: the values the plan may take, nplan and the largest stair height |h| (2 slab_half[2]); -2 as above. */
+int lhw_sim_footstep_limits(const lhw_sim* sim, int* nplan, double* max_height);
+int lhw_sim_reset_footsteps(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                            const int32_t* mode, const void* value, int fresh, void* obs, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

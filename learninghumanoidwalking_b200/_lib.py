@@ -38,6 +38,8 @@ SIGNATURES = {
     "lhw_sim_set_command": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 4),
     "lhw_sim_command_words": (c_int, []),
     "lhw_sim_command_accumulate": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 3),
+    "lhw_sim_footstep_limits": (c_int, [c_void_p] * 3),
+    "lhw_sim_reset_footsteps": (c_int, [c_void_p] * 3 + [c_int, c_uint32, c_uint32, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

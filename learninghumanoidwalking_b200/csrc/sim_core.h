@@ -2025,10 +2025,15 @@ template <class real, int NJ, int TK> LHW_DEV void step_update_goals(Work<real, 
     w.goal[6 + idx] = cy > (real)(4 * 2.220446049250313e-16) ? m_atan2(r10, r00) : (real)0;
   }
 }
+// a chosen footstep plan (lhw_sim_reset_footsteps, DESIGN.md §7.7): mode is an ST_* value and value the FORWARD signed stair
+// height (m), the LATERAL side c (+1 = the robot's left), the CURVED plan index (-1: drawn) or 0.  It replaces only the draws that
+// pick the plan; every other draw of the reset is the plain reset's
+template <class real> struct StepPlan { int mode; real value; };
+
 // SteppingTask.reset (:243-334); draws: stream 3 lane 0 mode, lane 1 phase, lane 2 first-step offset / plan index / lateral
-// sign, lane 3 randint(2,4); stream 4 lane 0 sign of the step height
-template <class real, int NJ, int TK>
-LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed) {
+// sign, lane 3 randint(2,4); stream 4 lane 0 sign of the step height.  PLAN: the plan is `plan`'s, not drawn
+template <class real, int NJ, int TK, bool PLAN = false>
+LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed, StepPlan<real> plan = {}) {
   uint32_t u[4], v[4];
   philox(seed, w.env_id, w.rng_ctr, 3, u);
   philox(seed, w.env_id, w.rng_ctr, 4, v);
@@ -2037,13 +2042,17 @@ LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m
   const real cm = u01<real>(u[0]);
   w.mode = cm < (real)0.15 ? ST_CURVED : cm < (real)(0.15 + 0.05) ? ST_STANDING : cm < (real)(0.15 + 0.05 + 0.2) ? ST_BACKWARD
            : cm < (real)(0.15 + 0.05 + 0.2 + 0.3) ? ST_LATERAL : ST_FORWARD;
+  if constexpr (PLAN) w.mode = plan.mode;
   real step_size = (real)0.3, step_height = 0;
   const real step_gap = (real)0.15;
   int num_steps = NSLAB;
   if (w.mode == ST_STANDING) num_steps = 1;
   else if (w.mode == ST_BACKWARD) step_size = (real)-0.1;
   else if (w.mode == ST_LATERAL) step_size = (real)0.4;
-  else if (w.mode == ST_FORWARD) step_height = randint(v[0], 2) == 0 ? -m.step_height : m.step_height;
+  else if (w.mode == ST_FORWARD) {
+    if constexpr (PLAN) step_height = plan.value;
+    else step_height = randint(v[0], 2) == 0 ? -m.step_height : m.step_height;
+  }
   // transform_sequence (:123-136): about the mid-point of the foot bodies, yawed with the root
   const real* R = w.xmat[0];
   const real cyn = m_sqrt(R[0] * R[0] + R[3] * R[3]);
@@ -2060,13 +2069,16 @@ LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m
     n++;
   };
   if (w.mode == ST_CURVED) {
-    const real* plan = m.plans + (size_t)randint(u[2], m.nplan) * PLAN_STRIDE;
-    const int len = (int)plan[0];
+    int k = randint(u[2], m.nplan);
+    if constexpr (PLAN) { if (plan.value >= 0 && plan.value < (real)m.nplan) k = (int)plan.value; }   // else the drawn plan
+    const real* pl = m.plans + (size_t)k * PLAN_STRIDE;
+    const int len = (int)pl[0];
 #pragma unroll 1
-    for (int i = 0; i < len; i++) put(plan[1 + 3 * i], plan[2 + 3 * i], 0, plan[3 + 3 * i]);
+    for (int i = 0; i < len; i++) put(pl[1 + 3 * i], pl[2 + 3 * i], 0, pl[3 + 3 * i]);
   } else if (w.mode == ST_LATERAL) {
     real y = 0;
-    const real c = randint(u[2], 2) == 0 ? (real)-1 : (real)1;
+    real c = randint(u[2], 2) == 0 ? (real)-1 : (real)1;
+    if constexpr (PLAN) c = plan.value;
 #pragma unroll 1
     for (int i = 1; i < num_steps; i++) {
       if (i % 2) y += step_size; else y -= (real)(2.0 / 3.0) * step_size;
@@ -2117,8 +2129,10 @@ LHW_DEV void terrain_repose(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m,
   }
 }
 
-// MujocoEnv.reset + BaseHumanoidEnv.reset_model + WalkingTask.reset
-template <class real, int NJ, int TK> LHW_DEV void env_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed) {
+// MujocoEnv.reset + BaseHumanoidEnv.reset_model + WalkingTask.reset.  PLAN (SteppingTask only): the footstep plan is `plan`
+template <class real, int NJ, int TK, bool PLAN = false>
+LHW_DEV void env_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed, StepPlan<real> plan = {}) {
+  static_assert(!PLAN || Cfg<NJ, TK>::STEP, "a footstep plan is a SteppingTask reset");
   constexpr int NV = 6 + 2 * NJ, NQ = NV + 1, NU = 2 * NJ;
   LHW_LANES(l) {
     if (l == 0) w.rng_ctr++;
@@ -2178,7 +2192,7 @@ template <class real, int NJ, int TK> LHW_DEV void env_reset(Work<real, NJ, TK>&
   LHW_LANES(l) {
     if (l == 0) {
       if constexpr (Cfg<NJ, TK>::STEP) {
-        step_task_reset<real, NJ, TK>(w, m, seed);
+        step_task_reset<real, NJ, TK, PLAN>(w, m, seed, plan);
       } else if constexpr (!Cfg<NJ, TK>::STAND) {
         uint32_t u[4];
         philox(seed, w.env_id, w.rng_ctr, 3, u);

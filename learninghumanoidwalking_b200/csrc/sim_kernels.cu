@@ -85,16 +85,25 @@ int fail(int code, const std::string& msg) {
     if (_e != cudaSuccess) return fail(-10, std::string(#call) + ": " + cudaGetErrorString(_e)); \
   } while (0)
 
-template <class real, int NJ, int TK>
+// PLAN (jvrc_step only, lhw_sim_reset_footsteps): env i resets with the footstep plan (plan_mode[i], plan_value[i]); rows whose
+// mode is not an ST_* value are skipped as masked-out rows are
+template <class real, int NJ, int TK, bool PLAN = false>
 __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, int32_t* __restrict__ state_i, int n_envs,
                                                     uint32_t seed, uint32_t first_id, const int32_t* __restrict__ mask,
-                                                    int fresh, real* __restrict__ obs_out) {
+                                                    int fresh, real* __restrict__ obs_out,
+                                                    const int32_t* __restrict__ plan_mode = nullptr,
+                                                    const real* __restrict__ plan_value = nullptr) {
   using W = Work<real, NJ, TK>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x;
   if (env >= n_envs) return;
   if (mask && !mask[env]) return;
+  StepPlan<real> plan = {};
+  if constexpr (PLAN) {
+    plan = {plan_mode[env], plan_value[env]};
+    if (plan.mode < ST_CURVED || plan.mode > ST_FORWARD) return;
+  }
   W& w = *reinterpret_cast<W*>(smem_raw);
   const Model<real, NJ, TK>& m = cmodel<real, NJ, TK>();
   constexpr int NR = Dims<real, NJ, TK>::NSTATE_R;
@@ -106,7 +115,7 @@ __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, i
     __syncwarp();
   }
   load_state<real, NJ, TK>(w, sr, si, first_id + env);
-  env_reset<real, NJ, TK>(w, m, seed);
+  env_reset<real, NJ, TK, PLAN>(w, m, seed, plan);
   store_state<real, NJ, TK>(w, sr, si);
   if (obs_out)
     for (int it = lane; it < W::NOBS; it += 32) obs_out[(size_t)env * W::NOBS + it] = w.obs[it];
@@ -240,6 +249,9 @@ struct lhw_sim {
   virtual int set_command(void* state_r, int32_t* state_i, int n_envs, const int32_t* mode, const void* ref, void* obs,
                           cudaStream_t st) = 0;
   virtual void command_accumulate(const void* state_r, int n_envs, const int32_t* done, double* acc, cudaStream_t st) = 0;
+  virtual int footstep_limits(int* nplan, double* max_height) const = 0;
+  virtual void reset_footsteps(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mode,
+                               const void* value, int fresh, void* obs, cudaStream_t st) = 0;
   virtual void set_step_height(double h) = 0;
 };
 
@@ -263,6 +275,9 @@ template <class real, int NJ, int TK> int prepare_variant(lhw_sim* s) {
   if (s->warps_per_block < 1) s->warps_per_block = 1;
   if ((int)s->work_bytes > maxsmem) return fail(-5, "working set does not fit in shared memory");
   if (prepare_kernel(step_kernel<real, NJ, TK>, s->work_bytes) || prepare_kernel(reset_kernel<real, NJ, TK>, s->work_bytes)) return -10;
+  if constexpr (Cfg<NJ, TK>::STEP) {
+    if (prepare_kernel(reset_kernel<real, NJ, TK, true>, s->work_bytes)) return -10;
+  }
   if (s->warps_per_block > 1 && prepare_kernel(step_kernel_mw<real, NJ, TK>, s->work_bytes * s->warps_per_block)) return -10;
   return 0;
 }
@@ -373,6 +388,24 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
 
   void command_accumulate(const void* state_r, int n_envs, const int32_t* done, double* acc, cudaStream_t st) override {
     command_accumulate_kernel<real, NJ, TK><<<(n_envs + 255) / 256, 256, 0, st>>>((const real*)state_r, n_envs, done, acc);
+  }
+
+  int footstep_limits(int* nplan, double* max_height) const override {
+    if constexpr (Cfg<NJ, TK>::STEP) {
+      *nplan = model.nplan;
+      *max_height = 2 * (double)model.slab_half[2];   // above it a slab's side face no longer covers the riser below the next slab
+      return 0;
+    } else {
+      return fail(-2, std::string(NJ == 5 ? (TK == 3 ? "h1_walk" : "h1") : TK == 2 ? "jvrc_walk_terrain" : "jvrc_walk") +
+                          " has no footstep plan: only jvrc_step (SteppingTask) takes one");
+    }
+  }
+
+  void reset_footsteps(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mode,
+                       const void* value, int fresh, void* obs, cudaStream_t st) override {
+    if constexpr (Cfg<NJ, TK>::STEP)
+      reset_kernel<real, NJ, TK, true><<<n_envs, 32, work_bytes, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, nullptr,
+                                                                       fresh, (real*)obs, mode, (const real*)value);
   }
 
   void set_step_height(double h) override {
@@ -510,6 +543,26 @@ int lhw_sim_set_command(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs,
   if (n_envs <= 0) return 0;
   const int rc = s->set_command(state_r, state_i, n_envs, mode, ref, obs, (cudaStream_t)stream);   // no model constants
   if (rc) return rc;
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_footstep_limits(const lhw_sim* s, int* nplan, double* max_height) {
+  if (!s || !nplan || !max_height) return fail(-1, "null argument");
+  return s->footstep_limits(nplan, max_height);
+}
+
+int lhw_sim_reset_footsteps(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                            const int32_t* mode, const void* value, int fresh, void* obs, void* stream) {
+  if (!s || !state_r || !state_i || !mode || !value) return fail(-1, "null argument");
+  int nplan = 0;
+  double max_height = 0;
+  if (const int rc = s->footstep_limits(&nplan, &max_height)) return rc;
+  if (n_envs <= 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (s->bind(st)) return -10;
+  s->reset_footsteps(state_r, state_i, n_envs, seed, first_env_id, mode, value, fresh, obs, st);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -170,6 +170,36 @@ void sim_command_accumulate(int64_t sim, const Tensor& state_r, const Tensor& do
   c10::cuda::CUDAGuard guard(I.device);
   ok(lhw_sim_command_accumulate(I.s, state_r.data_ptr(), (int)n, done.data_ptr<int32_t>(), acc.data_ptr<double>(), stream_of(state_r)),
      "lhw_sim_command_accumulate");
+}
+
+void sim_reset_footsteps(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const Tensor& mode,
+                         const Tensor& value, bool fresh, Tensor obs) {
+  const SimInfo I = sim_info(sim);
+  int nplan = 0;
+  double max_height = 0;
+  ok(lhw_sim_footstep_limits(I.s, &nplan, &max_height), "lhw_sim_reset_footsteps");   // names a variant without plans
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  check_cuda(mode, "mode", at::kInt, I.device); check_shape(mode, "mode", {n});
+  check_cuda(value, "value", I.real, I.device); check_shape(value, "value", {n});
+  check_cuda(obs, "obs", I.real, I.device); check_shape(obs, "obs", {n, I.nobs});
+  c10::cuda::CUDAGuard guard(I.device);
+  // called once per evaluation, outside graphs: the host syncs on the values are affordable
+  TORCH_CHECK(!((mode < -1) | (mode > 4)).any().item<bool>(),
+              "lhw: mode must be -1 (untouched), 0 (CURVED), 1 (STANDING), 2 (BACKWARD), 3 (LATERAL) or 4 (FORWARD)");
+  TORCH_CHECK(value.isfinite().all().item<bool>(), "lhw: value must be finite");
+  const Tensor v = value.to(at::kDouble);
+  TORCH_CHECK(!((mode == 4) & (v.abs() > max_height)).any().item<bool>(), "lhw: a FORWARD stair height must lie in [-", max_height,
+              ", ", max_height, "] m (2 slab_half[2]: above it a slab's side face no longer covers the riser below the next slab)");
+  TORCH_CHECK(!((mode == 3) & (v != 1) & (v != -1)).any().item<bool>(), "lhw: a LATERAL value must be +1 (left) or -1 (right)");
+  TORCH_CHECK(!((mode == 0) & (v != -1) & ((v < 0) | (v >= nplan) | (v != v.floor()))).any().item<bool>(),
+              "lhw: a CURVED value must be -1 (drawn) or a plan index in [0, ", nplan, ")");
+  TORCH_CHECK(!(((mode == 1) | (mode == 2)) & (v != 0)).any().item<bool>(), "lhw: a STANDING or BACKWARD value must be 0");
+  ok(lhw_sim_reset_footsteps(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                             mode.data_ptr<int32_t>(), value.data_ptr(), fresh ? 1 : 0, obs.data_ptr(), stream_of(state_r)),
+     "lhw_sim_reset_footsteps");
 }
 
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
@@ -377,6 +407,8 @@ TORCH_LIBRARY(lhw, m) {
         "Tensor? d) -> ()");
   m.def("sim_set_command(int sim, Tensor(a!) state_r, Tensor(b!) state_i, Tensor mode, Tensor ref, Tensor(c!) obs) -> ()");
   m.def("sim_command_accumulate(int sim, Tensor state_r, Tensor done, Tensor(a!) acc) -> ()");
+  m.def("sim_reset_footsteps(int sim, Tensor(a!) state_r, Tensor(b!) state_i, int seed, int first_env_id, Tensor mode, Tensor value, "
+        "bool fresh, Tensor(c!) obs) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -410,6 +442,7 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_push", &sim_push);
   m.impl("sim_set_command", &sim_set_command);
   m.impl("sim_command_accumulate", &sim_command_accumulate);
+  m.impl("sim_reset_footsteps", &sim_reset_footsteps);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

@@ -28,6 +28,9 @@ STEP_REWARD_NAMES = ("foot_frc_score", "foot_vel_score", "orient_cost", "height_
 # (csrc/sim_core.h MODE_HELD)
 COMMAND_ENVS = ("jvrc_walk", "jvrc_walk_terrain", "h1_walk")
 MODE_HELD = 1 << 30
+# chosen footstep plans (reset_footsteps, DESIGN.md §7.7): the SteppingTask's plan types in the order of the kernel's mode word
+# (csrc/sim_core.h ST_*)
+FOOTSTEP_MODES = ("CURVED", "STANDING", "BACKWARD", "LATERAL", "FORWARD")
 N_REWARD_SLOTS = 10   # width of the kernel's reward-term record (csrc/sim_core.h NREW); unused slots are 0
 # h1_walk (DESIGN.md §4.6): joints (hip_yaw, hip_roll, hip_pitch, knee, ankle), left leg then right.  The mirror swaps the legs and
 # negates yaw and roll; in the observation also the root roll and the x, z angular velocities.  The 8 walking-task words map to
@@ -270,6 +273,48 @@ class BatchedHumanoidEnv:
             raise ValueError("ref must be finite")
         _lib.ops().sim_set_command(self._h.value, self.state_r, self.state_i, mode.to(device=self.device, dtype=torch.int32),
                                    ref.to(device=self.device, dtype=self.dtype), self.obs)
+
+    def footstep_limits(self) -> tuple[int, float]:
+        """(number of curved plans, largest FORWARD stair height |h| in m) that reset_footsteps accepts: the plans of
+        model/jvrc_step.json, and twice a slab's half height (above it a slab's side face no longer covers the riser below the next
+        slab)."""
+        if self.model_name != "jvrc_step":
+            raise ValueError(f"{self.model_name} has no footstep plan: only jvrc_step (SteppingTask) takes one")
+        st = self.mj["stepping"]
+        return len(st["plans"]), 2 * float(st["slab_half"][2])
+
+    def reset_footsteps(self, mode, value) -> torch.Tensor:
+        """Reset environments with a chosen stepping-stone plan; returns self.obs.  mode [N] holds per env -1 (untouched) or a plan
+        type of FOOTSTEP_MODES (0 CURVED, 1 STANDING, 2 BACKWARD, 3 LATERAL, 4 FORWARD), value [N] its value: FORWARD the signed
+        stair height in m, LATERAL +1 (to the robot's left) or -1, CURVED a plan index or -1 (the reset's own draw), STANDING and
+        BACKWARD 0; sequences or tensors.  Every other draw of the reset is the plain reset's, and the plan lasts for the episode
+        (include/lhw_b200.h: lhw_sim_reset_footsteps).  On a fresh env every row needs a plan."""
+        nplan, max_h = self.footstep_limits()
+        mode = torch.as_tensor(mode).detach().to("cpu").reshape(-1)
+        value = torch.as_tensor(value, dtype=torch.float64).detach().to("cpu").reshape(-1)
+        if mode.dtype.is_floating_point or mode.dtype == torch.bool or mode.shape != (self.num_envs,):
+            raise ValueError(f"mode must hold {self.num_envs} integers, got {tuple(mode.shape)} of {mode.dtype}")
+        if value.shape != (self.num_envs,):
+            raise ValueError(f"value must hold {self.num_envs} numbers, got {tuple(value.shape)}")
+        if ((mode < -1) | (mode > 4)).any():
+            raise ValueError(f"mode must be -1 (untouched) or 0..4 ({', '.join(FOOTSTEP_MODES)}), got {sorted(set(mode.tolist()))}")
+        if not torch.isfinite(value).all():
+            raise ValueError("value must be finite")
+        if ((mode == 4) & (value.abs() > max_h)).any():
+            raise ValueError(f"a FORWARD stair height must lie in [-{max_h:g}, {max_h:g}] m")
+        if ((mode == 3) & (value != 1) & (value != -1)).any():
+            raise ValueError("a LATERAL value must be +1 (left) or -1 (right)")
+        if ((mode == 0) & (value != -1) & ((value < 0) | (value >= nplan) | (value != value.floor()))).any():
+            raise ValueError(f"a CURVED value must be -1 (drawn) or a plan index in [0, {nplan})")
+        if (((mode == 1) | (mode == 2)) & (value != 0)).any():
+            raise ValueError("a STANDING or BACKWARD value must be 0")
+        if self._fresh and (mode < 0).any():
+            raise ValueError("this env has never been reset: give every row a plan, or call reset() first")
+        _lib.ops().sim_reset_footsteps(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id,
+                                       mode.to(device=self.device, dtype=torch.int32), value.to(device=self.device, dtype=self.dtype),
+                                       self._fresh, self.obs)
+        self._fresh = False
+        return self.obs
 
     def command_accumulate(self, acc: torch.Tensor) -> torch.Tensor:
         """Add the last control step (taken with autoreset=False) to the command sweep's signed-velocity records acc, a

@@ -14,6 +14,10 @@ from the same accumulator words: fell before the push (EV_DONE set and EV_LEN <=
 The command-tracking sweep (`eval --num-envs N --command forward:0,0.2 inplace:0.4 standing`, DESIGN.md §7.6) gives env i the held
 command of cell i mod C (BatchedHumanoidEnv.set_command) after the reset, before the first step and outside the graph.  The graph
 body then also launches BatchedHumanoidEnv.command_accumulate, whose per-env records give the signed mean velocities of each cell.
+
+The footstep sweep (`eval --num-envs N --footsteps forward:0,0.05,0.1 lateral:left,right curved standing`, DESIGN.md §7.7, jvrc_step)
+resets env i with the stepping-stone plan of cell i mod C (BatchedHumanoidEnv.reset_footsteps) in place of the one plain reset.  The
+graph body is unchanged: the accumulator's footsteps-reached and sequence-length words already give each cell's progress.
 """
 from __future__ import annotations
 
@@ -21,6 +25,8 @@ import json
 
 import numpy as np
 import torch
+
+from ..envs.batched_env import FOOTSTEP_MODES
 
 # the accumulator words of csrc/sim_core.h (EV_*), per env
 LEN, RET, DONE, TERMS, TRACK, REACHED, SEQLEN, WORDS = 0, 1, 2, 3, 13, 25, 26, 27
@@ -58,21 +64,32 @@ def command_refs(mode: np.ndarray, value: np.ndarray) -> np.ndarray:
     return ref
 
 
+def footstep_grid(n: int, cells):
+    """Per env (plan type index, value) of the footstep sweep: env i is in cell i mod C of cells = [(plan type name, value), ...]."""
+    c = np.arange(n) % len(cells)
+    return (np.asarray([FOOTSTEP_MODES.index(m) for m, _ in cells], dtype=np.int32)[c],
+            np.asarray([v for _, v in cells], dtype=np.float64)[c])
+
+
 @torch.no_grad()
-def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None):
+def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None):
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
     [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
     push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
     change d [N, 2] (BatchedHumanoidEnv.push); with push=None nothing but the control steps is launched.
     command = (mode [N], ref [N, 3]): held commands (BatchedHumanoidEnv.set_command) applied after the reset, and every step also
-    adds to the [N, C_WORDS] signed-velocity records; then the return is (accumulators, signed-velocity records)."""
+    adds to the [N, C_WORDS] signed-velocity records; then the return is (accumulators, signed-velocity records).
+    footsteps = (mode [N], value [N]): the reset is BatchedHumanoidEnv.reset_footsteps with these plans instead of reset()."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
     if command is not None and env.command_words() != C_WORDS:
         raise RuntimeError(f"the library's command record has {env.command_words()} words, this module knows {C_WORDS}")
     acc = torch.zeros(env.num_envs, WORDS, dtype=torch.float64, device=env.device)
     cacc = torch.zeros(env.num_envs, C_WORDS, dtype=torch.float64, device=env.device) if command is not None else None
-    env.reset()
+    if footsteps is not None:
+        env.reset_footsteps(*footsteps)
+    else:
+        env.reset()
     if command is not None:
         env.set_command(*command)
     state = env.obs.float().clone()
@@ -224,6 +241,38 @@ def format_command_table(c: dict) -> str:
     return "\n".join(lines)
 
 
+def footstep_label(name: str, value: float) -> str:
+    """The cell as the command line writes it: forward:0.1, lateral:left, curved:17, curved (drawn), standing, backward."""
+    if name == "LATERAL":
+        return "lateral:" + ("left" if value > 0 else "right")
+    if name == "FORWARD" or (name == "CURVED" and value >= 0):
+        return f"{name.lower()}:{value:g}"
+    return name.lower()
+
+
+def footstep_summary(acc: np.ndarray, mode: np.ndarray, value: np.ndarray, cells) -> dict:
+    """The footstep sweep's outcome per cell: n, fall fraction, mean episode length, mean footsteps reached and mean sequence
+    length, completed fraction (reached >= sequence length - 1, as summarize counts it) and the mean return."""
+    out = []
+    for name, val in cells:
+        m = (mode == FOOTSTEP_MODES.index(name)) & (value == float(val))
+        reached, seq_len = acc[m, REACHED], acc[m, SEQLEN]
+        out.append(dict(mode=name, value=float(val), label=footstep_label(name, float(val)), n=int(m.sum()),
+                        fall_fraction=float((acc[m, DONE] != 0).mean()), mean_length=float(acc[m, LEN].mean()),
+                        mean_reached=float(reached.mean()), mean_sequence_length=float(seq_len.mean()),
+                        completed_fraction=float((reached >= seq_len - 1).mean()), return_mean=float(acc[m, RET].mean())))
+    return dict(cells=out)
+
+
+def format_footstep_table(f: dict) -> str:
+    lines = ["  chosen footstep plans: reached = mean footsteps reached of the mean sequence length",
+             "    plan                 n   fell  length     reached  completed    return"]
+    for x in f["cells"]:
+        lines.append(f"    {x['label']:<16s} {x['n']:>5d} {x['fall_fraction']:6.3f} {x['mean_length']:7.1f}  "
+                     f"{x['mean_reached']:5.2f}/{x['mean_sequence_length']:<5.2f} {x['completed_fraction']:8.3f} {x['return_mean']:9.3f}")
+    return "\n".join(lines)
+
+
 def format_table(s: dict, max_traj_len: int) -> str:
     L = s["length"]
     lines = [f"{s['num_envs']} environments, one episode each, horizon {max_traj_len} control steps",
@@ -244,14 +293,17 @@ def format_table(s: dict, max_traj_len: int) -> str:
     return "\n".join(lines)
 
 
-def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None) -> dict:
+def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None,
+                     footsteps=None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
     out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
     push-recovery sweep, with its table and `summary.push`.  commands = [(mode name, value), ...]: the command-tracking sweep
-    (env i holds the command of cell i mod len(commands)), with its table and `summary.commands`.  Returns the report."""
-    if push is not None and commands is not None:
-        raise ValueError("the push sweep and the command sweep are separate evaluations")
-    sweep = held = None
+    (env i holds the command of cell i mod len(commands)), with its table and `summary.commands`.  footsteps = [(plan type name,
+    value), ...]: the footstep sweep (env i resets with the plan of cell i mod len(footsteps)), with its table and
+    `summary.footsteps_sweep`.  Returns the report."""
+    if sum(x is not None for x in (push, commands, footsteps)) > 1:
+        raise ValueError("the push sweep, the command sweep and the footstep sweep are separate evaluations")
+    sweep = held = plans = None
     if push is not None:
         k = int(round(push["push_at"] / env.dt))
         speed, dir_deg = push_grid(env.num_envs, push["speeds"], push["directions"])
@@ -259,7 +311,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
     if commands is not None:
         cmd_mode, cmd_value = command_grid(env.num_envs, commands)
         held = (cmd_mode, command_refs(cmd_mode, cmd_value))
-    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held)
+    if footsteps is not None:
+        fs_mode, fs_value = footstep_grid(env.num_envs, footsteps)
+        plans = (fs_mode, fs_value)
+    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans)
     acc, cacc = (out[0].cpu().numpy(), out[1].cpu().numpy()) if commands is not None else (out.cpu().numpy(), None)
     summary = summarize(acc, env.model_name, env.reward_names)
     pe = per_env(acc, env.model_name, env.reward_names)
@@ -274,6 +329,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
                   command_steps=cacc[:, C_LEN].astype(int).tolist(), v_fwd_sum=cacc[:, C_VF].tolist(),
                   v_lat_sum=cacc[:, C_VL].tolist(), yaw_rate_sum=cacc[:, C_WZ].tolist())
         print(format_command_table(summary["commands"]))
+    if footsteps is not None:
+        summary["footsteps_sweep"] = footstep_summary(acc, fs_mode, fs_value, footsteps)
+        pe.update(footstep_mode=[FOOTSTEP_MODES[m] for m in fs_mode], footstep_value=fs_value.tolist())
+        print(format_footstep_table(summary["footsteps_sweep"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
                   max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:

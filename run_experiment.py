@@ -25,7 +25,10 @@ env once, at --push-at seconds, with the speed and direction of its cell of the 
 prints the survival of each cell; the batched evaluation never gets the training pushes.  `eval --command forward:0,0.2,0.4
 inplace:-0.4,0.4 standing` holds walking commands (DESIGN §7.6): with --num-envs N env i holds the command of cell i mod C and the
 run prints the achieved velocities and tracking errors of each cell; without it, the one command is held on the single-env roll-out
-(and its video) and re-applied after every reset there.
+(and its video) and re-applied after every reset there.  `eval --footsteps forward:0,0.05,0.1 lateral:left,right backward curved
+standing` chooses jvrc_step's stepping-stone plans (DESIGN §7.7): with --num-envs N env i resets with the plan of cell i mod C and the
+run prints the falls and footsteps reached of each cell; without it, the one plan is chosen at every reset of the single-env
+roll-out (and its video).
 """
 import argparse
 import os
@@ -88,7 +91,12 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
               # held walking commands (DESIGN §7.6)
               ("--command", dict(type=_S, nargs="+", action="extend", default=None,
                                  help="held walking commands MODE[:v1,v2,...]: forward:V m/s, inplace:W rad/s, standing; with "
-                                      "--num-envs one cell per (mode, value), else exactly one"))]
+                                      "--num-envs one cell per (mode, value), else exactly one")),
+              # chosen stepping-stone plans of jvrc_step (DESIGN §7.7)
+              ("--footsteps", dict(type=_S, nargs="+", action="extend", default=None,
+                                   help="jvrc_step footstep plans TYPE[:v1,v2,...]: forward:H (signed stair height, m), "
+                                        "lateral:left,right, curved[:plan index,...], backward, standing; with --num-envs one cell "
+                                        "per (type, value), else exactly one"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -376,6 +384,62 @@ def check_command_env(env_name):
         raise SystemExit(f"eval --command: the run's env {env_name} has no walking command; only {', '.join(COMMAND_ENVS)} take one")
 
 
+def footstep_cells(args):
+    """The chosen plans of `eval --footsteps ...` as [(plan type name, value), ...] (envs/batched_env.py FOOTSTEP_MODES), or None
+    without the flag; refuses a list that cannot be run before anything is loaded.  Bare `curved` is a curved plan drawn at the
+    reset (value -1)."""
+    if args.footsteps is None:
+        return None
+    from learninghumanoidwalking_b200.model import load_model
+    st = load_model("jvrc_step")["stepping"]
+    nplan, max_h = len(st["plans"]), 2 * float(st["slab_half"][2])
+    cells = []
+    for spec in args.footsteps:
+        name, sep, values = spec.partition(":")
+        if name not in ("forward", "lateral", "curved", "backward", "standing"):
+            raise SystemExit(f"eval --footsteps {spec!r}: unknown plan type {name!r}; expected forward:H[,H...], lateral:left,right, "
+                             "curved[:I,...], backward or standing")
+        if name in ("backward", "standing") or (name == "curved" and not sep):
+            if sep:
+                raise SystemExit(f"eval --footsteps {spec!r}: {name} takes no values")
+            cells.append((name.upper(), -1.0 if name == "curved" else 0.0))
+            continue
+        if name == "lateral":
+            sides = values.split(",")
+            if not all(v in ("left", "right") for v in sides):
+                raise SystemExit(f"eval --footsteps {spec!r}: expected lateral:left, lateral:right or lateral:left,right")
+            cells += [("LATERAL", 1.0 if v == "left" else -1.0) for v in sides]
+            continue
+        try:
+            vs = [float(v) for v in values.split(",")]
+        except ValueError:
+            raise SystemExit(f"eval --footsteps {spec!r}: expected {name}:" +
+                             ("H[,H...] with comma-separated stair heights in m" if name == "forward" else "I[,I...] with plan indices"))
+        if not all(abs(v) < float("inf") for v in vs):
+            raise SystemExit(f"eval --footsteps {spec!r}: every value must be finite")
+        if name == "forward" and any(abs(v) > max_h for v in vs):
+            raise SystemExit(f"eval --footsteps {spec!r}: a stair height must lie in [-{max_h:g}, {max_h:g}] m (twice a slab's half "
+                             "height: above it a slab's side face no longer covers the riser below the next slab)")
+        if name == "curved" and any(v != int(v) or not 0 <= v < nplan for v in vs):
+            raise SystemExit(f"eval --footsteps {spec!r}: a curved plan index must be an integer in [0, {nplan})")
+        cells += [(name.upper(), v) for v in vs]
+    if args.push_speeds is not None or args.command is not None:
+        raise SystemExit("eval --footsteps, --command and --push-speeds are separate sweeps: run them one at a time")
+    if args.num_envs is None and len(cells) > 1:
+        raise SystemExit(f"eval --footsteps: {len(cells)} plans need the batched evaluation (add --num-envs N); the single-env "
+                         "roll-out takes exactly one")
+    if args.num_envs is not None and args.num_envs < len(cells):
+        raise SystemExit(f"eval --num-envs {args.num_envs}: --footsteps lists {len(cells)} cells, and every cell needs at least one "
+                         "environment")
+    return cells
+
+
+def check_footstep_env(env_name):
+    """Refuse --footsteps for a run whose env is not jvrc_step, before its actor is loaded."""
+    if env_name != "jvrc_step":
+        raise SystemExit(f"eval --footsteps: the run's env {env_name} has no footstep plan; only jvrc_step (SteppingTask) takes one")
+
+
 def evaluate_batched(args):
     """`eval --num-envs N`: the deterministic actor on N environments of the run's env, horizon and YAML, one episode each
     (rl/evaluation.py), with a table of the outcomes and, with --report, the JSON report."""
@@ -385,12 +449,15 @@ def evaluate_batched(args):
         raise SystemExit("eval --out-dir renders one roll-out to video; it cannot be combined with --num-envs")
     push = push_sweep(args)
     commands = command_cells(args)
+    footsteps = footstep_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
         run_args = pickle.load(f)
     if commands is not None:
         check_command_env(run_args.env)
+    if footsteps is not None:
+        check_footstep_env(run_args.env)
     yaml = run_args.yaml
     if yaml is not None and Path(path_to_actor.parent, Path(yaml).name).exists():
         yaml = str(Path(path_to_actor.parent, Path(yaml).name))      # the copy that rode along with the run, as `resume` uses
@@ -412,7 +479,8 @@ def evaluate_batched(args):
     precision = 64 if args.precision is None else args.precision
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
-    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands)
+    report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands,
+                 footsteps=footsteps)
     env.close()
     return report
 
@@ -426,12 +494,15 @@ def evaluate(args):
     if args.push_speeds is not None or args.push_directions is not None or args.push_at is not None:
         raise SystemExit("eval --push-speeds, --push-directions and --push-at belong to the batched evaluation: add --num-envs N")
     commands = command_cells(args)
+    footsteps = footstep_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
         run_args = pickle.load(f)
     if commands is not None:
         check_command_env(run_args.env)
+    if footsteps is not None:
+        check_footstep_env(run_args.env)
     cv2 = None
     if args.out_dir is not None:
         try:
@@ -446,7 +517,11 @@ def evaluate(args):
     env = import_env(run_args.env)(1, precision=64, seed=args.seed or 0)
 
     def reset():
-        env.reset()
+        if footsteps is not None:     # the one plan, chosen again at every reset
+            from learninghumanoidwalking_b200.rl.evaluation import footstep_grid
+            env.reset_footsteps(*footstep_grid(1, footsteps))
+        else:
+            env.reset()
         if commands is not None:     # the one command, held again after every reset
             from learninghumanoidwalking_b200.rl.evaluation import command_grid, command_refs
             mode, value = command_grid(1, commands)
