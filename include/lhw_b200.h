@@ -142,6 +142,21 @@ int lhw_sim_footstep_limits(const lhw_sim* sim, int* nplan, double* max_height);
 int lhw_sim_reset_footsteps(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
                             const int32_t* mode, const void* value, int fresh, void* obs, void* stream);
 
+/* lhw_sim_step_stairs / lhw_sim_reset_stairs: lhw_sim_step / lhw_sim_reset with a stair curriculum per env (DESIGN.md §7.8;
+ * legged_gym's terrain levels).  jvrc_step only; the other variants are refused with -2 and a message that names them, as is
+ * n_levels outside 2..21.  level [n] (device int32) holds each env's level L, clamped to [0, n_levels) where it is read.  Every reset
+ * these launches do builds a FORWARD plan with the stair magnitude (real)(0.01 L) in place of the sim-wide step height; its sign
+ * and every other draw are the plain reset's.  lhw_sim_step_stairs with autoreset != 0 moves the level of an env whose ended
+ * episode was a FORWARD one, just before its reset: r = footstep targets reached, n = sequence length, fell = done; L + 1 (at most
+ * n_levels - 1) if !fell and 2 r >= n, L - 1 (at least 0) if fell and 2 r < n, else unchanged.  Nothing else writes level;
+ * lhw_sim_reset_stairs only reads it. */
+int lhw_sim_reset_stairs(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                         const int32_t* mask, int fresh, void* obs, const int32_t* level, int n_levels, void* stream);
+int lhw_sim_step_stairs(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                        const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
+                        void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, int32_t* level, int n_levels,
+                        void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

@@ -40,6 +40,11 @@ SIGNATURES = {
     "lhw_sim_command_accumulate": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 3),
     "lhw_sim_footstep_limits": (c_int, [c_void_p] * 3),
     "lhw_sim_reset_footsteps": (c_int, [c_void_p] * 3 + [c_int, c_uint32, c_uint32, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "lhw_sim_reset_stairs": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, c_int, c_void_p, c_void_p,
+                                     c_int, c_void_p]),
+    "lhw_sim_step_stairs": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, c_int, c_int,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                    c_void_p]),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

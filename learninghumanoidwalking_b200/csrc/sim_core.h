@@ -2030,10 +2030,27 @@ template <class real, int NJ, int TK> LHW_DEV void step_update_goals(Work<real, 
 // pick the plan; every other draw of the reset is the plain reset's
 template <class real> struct StepPlan { int mode; real value; };
 
+// the stair curriculum (lhw_sim_step_stairs / lhw_sim_reset_stairs, DESIGN.md §7.8): env i has a level L in [0, n_levels), and its
+// FORWARD plans climb or descend stairs of 0.01 L m.  Levels outside the range are clamped on read
+enum { STAIR_MAX_LEVELS = 21 };   // 0 .. 0.2 m = 2 slab_half[2], the largest stair a chosen plan may have (lhw_sim_footstep_limits)
+LHW_DEV int stair_level_clamp(int level, int n_levels) { return level < 0 ? 0 : level >= n_levels ? n_levels - 1 : level; }
+// the magnitude lhw_sim_set_step_height(0.01 L) would store
+template <class real> LHW_DEV real stair_level_height(int level) { return (real)(0.01 * level); }
+// the level after an ended FORWARD episode that reached target `reached` of a sequence of `seq_len`: up one if it did not fall and
+// reached half the sequence, down one if it fell short of half, else unchanged
+template <class real> LHW_DEV int stair_level_next(int level, int n_levels, int fell, real reached, real seq_len) {
+  const bool far = 2 * reached >= seq_len;
+  if (!fell && far) return level + 1 < n_levels ? level + 1 : n_levels - 1;
+  if (fell && !far) return level > 0 ? level - 1 : 0;
+  return level;
+}
+
 // SteppingTask.reset (:243-334); draws: stream 3 lane 0 mode, lane 1 phase, lane 2 first-step offset / plan index / lateral
-// sign, lane 3 randint(2,4); stream 4 lane 0 sign of the step height.  PLAN: the plan is `plan`'s, not drawn
-template <class real, int NJ, int TK, bool PLAN = false>
-LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed, StepPlan<real> plan = {}) {
+// sign, lane 3 randint(2,4); stream 4 lane 0 sign of the step height.  PLAN: the plan is `plan`'s, not drawn.  STAIRS: a FORWARD
+// plan's stair magnitude is `stair` (the env's curriculum level), not the sim-wide m.step_height; its sign is still drawn
+template <class real, int NJ, int TK, bool PLAN = false, bool STAIRS = false>
+LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed, StepPlan<real> plan = {},
+                             real stair = 0) {
   uint32_t u[4], v[4];
   philox(seed, w.env_id, w.rng_ctr, 3, u);
   philox(seed, w.env_id, w.rng_ctr, 4, v);
@@ -2051,6 +2068,7 @@ LHW_DEV void step_task_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m
   else if (w.mode == ST_LATERAL) step_size = (real)0.4;
   else if (w.mode == ST_FORWARD) {
     if constexpr (PLAN) step_height = plan.value;
+    else if constexpr (STAIRS) step_height = randint(v[0], 2) == 0 ? -stair : stair;
     else step_height = randint(v[0], 2) == 0 ? -m.step_height : m.step_height;
   }
   // transform_sequence (:123-136): about the mid-point of the foot bodies, yawed with the root
@@ -2129,10 +2147,12 @@ LHW_DEV void terrain_repose(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m,
   }
 }
 
-// MujocoEnv.reset + BaseHumanoidEnv.reset_model + WalkingTask.reset.  PLAN (SteppingTask only): the footstep plan is `plan`
-template <class real, int NJ, int TK, bool PLAN = false>
-LHW_DEV void env_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed, StepPlan<real> plan = {}) {
+// MujocoEnv.reset + BaseHumanoidEnv.reset_model + WalkingTask.reset.  PLAN (SteppingTask only): the footstep plan is `plan`.
+// STAIRS (SteppingTask only): a FORWARD plan's stair magnitude is `stair`
+template <class real, int NJ, int TK, bool PLAN = false, bool STAIRS = false>
+LHW_DEV void env_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint32_t seed, StepPlan<real> plan = {}, real stair = 0) {
   static_assert(!PLAN || Cfg<NJ, TK>::STEP, "a footstep plan is a SteppingTask reset");
+  static_assert(!STAIRS || Cfg<NJ, TK>::STEP, "a stair curriculum is a SteppingTask reset");
   constexpr int NV = 6 + 2 * NJ, NQ = NV + 1, NU = 2 * NJ;
   LHW_LANES(l) {
     if (l == 0) w.rng_ctr++;
@@ -2192,7 +2212,7 @@ LHW_DEV void env_reset(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, uint
   LHW_LANES(l) {
     if (l == 0) {
       if constexpr (Cfg<NJ, TK>::STEP) {
-        step_task_reset<real, NJ, TK, PLAN>(w, m, seed, plan);
+        step_task_reset<real, NJ, TK, PLAN, STAIRS>(w, m, seed, plan, stair);
       } else if constexpr (!Cfg<NJ, TK>::STAND) {
         uint32_t u[4];
         philox(seed, w.env_id, w.rng_ctr, 3, u);
@@ -2218,11 +2238,14 @@ struct StepOut {
   int32_t* done; int32_t* ended; int32_t* ep_len; void* ep_rew;
 };
 
-// BaseHumanoidEnv.step + the RolloutWorker's bookkeeping (traj_len truncation, auto-reset, episode stats)
-template <class real, int NJ, int TK>
+// BaseHumanoidEnv.step + the RolloutWorker's bookkeeping (traj_len truncation, auto-reset, episode stats).  STAIRS (SteppingTask
+// only, DESIGN.md §7.8): *level is the env's stair-curriculum level of n_levels; an auto-reset first moves it by the ending episode
+// when that was a FORWARD one (stair_level_next), then resets with its stair height
+template <class real, int NJ, int TK, bool STAIRS = false>
 LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const real* action, uint32_t seed, int max_traj_len,
                       int autoreset, const int block_sync, const int alive, real* obs_out, real* term_obs_out, real* reward_out, real* rew_terms_out,
-                      int32_t* done_out, int32_t* ended_out, int32_t* ep_len_out, real* ep_rew_out) {
+                      int32_t* done_out, int32_t* ended_out, int32_t* ep_len_out, real* ep_rew_out, int32_t* level = nullptr,
+                      int n_levels = 0) {
   constexpr int NU = 2 * NJ, NOBS = Work<real, NJ, TK>::NOBS;
   // action smoothing + nominal offsets (base_humanoid_env.py:209-212, robot_base.py:80-85)
   // one event counter per control step: every draw of this step is keyed by rng_ctr + 1 (stored below)
@@ -2478,14 +2501,23 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
     }
   }
   if (ended && autoreset) {
+    real stair = 0;   // STAIRS: the next episode's stair magnitude (lane 0's, the lane that builds the plan)
     LHW_LANES(l) {
       if (l == 0) {
         if (ep_len_out) ep_len_out[0] = w.ep_len;
         if (ep_rew_out) ep_rew_out[0] = w.ep_rew;
+        if constexpr (STAIRS) {
+          int lv = stair_level_clamp(level[0], n_levels);
+          if (w.mode == ST_FORWARD) {
+            lv = stair_level_next<real>(lv, n_levels, done, w.tk[1], w.tk[0]);
+            level[0] = lv;
+          }
+          stair = stair_level_height<real>(lv);
+        }
       }
     }
     LHW_SYNC();
-    env_reset<real, NJ, TK>(w, m, seed);
+    env_reset<real, NJ, TK, false, STAIRS>(w, m, seed, {}, stair);
   }
   LHW_LANES(l) {
     for (int it = l; it < NOBS; it += 32) obs_out[it] = w.obs[it];

@@ -86,13 +86,15 @@ int fail(int code, const std::string& msg) {
   } while (0)
 
 // PLAN (jvrc_step only, lhw_sim_reset_footsteps): env i resets with the footstep plan (plan_mode[i], plan_value[i]); rows whose
-// mode is not an ST_* value are skipped as masked-out rows are
-template <class real, int NJ, int TK, bool PLAN = false>
+// mode is not an ST_* value are skipped as masked-out rows are.  STAIRS (jvrc_step only, lhw_sim_reset_stairs): a FORWARD plan of
+// env i has the stair magnitude of its curriculum level level[i] of n_levels
+template <class real, int NJ, int TK, bool PLAN = false, bool STAIRS = false>
 __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, int32_t* __restrict__ state_i, int n_envs,
                                                     uint32_t seed, uint32_t first_id, const int32_t* __restrict__ mask,
                                                     int fresh, real* __restrict__ obs_out,
                                                     const int32_t* __restrict__ plan_mode = nullptr,
-                                                    const real* __restrict__ plan_value = nullptr) {
+                                                    const real* __restrict__ plan_value = nullptr,
+                                                    const int32_t* __restrict__ level = nullptr, int n_levels = 0) {
   using W = Work<real, NJ, TK>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -115,7 +117,9 @@ __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, i
     __syncwarp();
   }
   load_state<real, NJ, TK>(w, sr, si, first_id + env);
-  env_reset<real, NJ, TK, PLAN>(w, m, seed, plan);
+  real stair = 0;
+  if constexpr (STAIRS) stair = stair_level_height<real>(stair_level_clamp(level[env], n_levels));
+  env_reset<real, NJ, TK, PLAN, STAIRS>(w, m, seed, plan, stair);
   store_state<real, NJ, TK>(w, sr, si);
   if (obs_out)
     for (int it = lane; it < W::NOBS; it += 32) obs_out[(size_t)env * W::NOBS + it] = w.obs[it];
@@ -124,13 +128,15 @@ __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, i
 // ONE warp per block: the warp's Work struct then sits at a link-time-constant shared-memory address, so every
 // access is [index + immediate] and no base register has to be kept (or rematerialised).  fp32: 28 blocks/SM (register
 // bound: 28 x 132 = 3696 environments at once on an H100, so a 4096-env batch is two waves); fp64: 16 blocks/SM (shared-memory bound).
-template <class real, int NJ, int TK>
+// STAIRS (jvrc_step only, lhw_sim_step_stairs): level [n_envs] holds the envs' stair-curriculum levels of n_levels, moved and used
+// by the auto-resets (sim_core.h env_step)
+template <class real, int NJ, int TK, bool STAIRS = false>
 __global__ void __launch_bounds__(32, sizeof(real) == 4 ? (Cfg<NJ, TK>::SLABS ? 24 : 28) : (Cfg<NJ, TK>::SLABS ? 12 : (NJ == NJ_JVRC ? 16 : 15)))
     step_kernel(real* __restrict__ state_r, int32_t* __restrict__ state_i, int n_envs, uint32_t seed, uint32_t first_id,
                 const real* __restrict__ actions, int max_traj_len, int autoreset, real* __restrict__ obs,
                 real* __restrict__ term_obs, real* __restrict__ reward, real* __restrict__ rew_terms,
                 int32_t* __restrict__ done, int32_t* __restrict__ ended, int32_t* __restrict__ ep_len,
-                real* __restrict__ ep_rew) {
+                real* __restrict__ ep_rew, int32_t* __restrict__ level = nullptr, int n_levels = 0) {
   using W = Work<real, NJ, TK>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int env = blockIdx.x;
@@ -141,16 +147,16 @@ __global__ void __launch_bounds__(32, sizeof(real) == 4 ? (Cfg<NJ, TK>::SLABS ? 
   real* sr = state_r + (size_t)env * NR;
   int32_t* si = state_i + (size_t)env * NSTATE_I;
   load_state<real, NJ, TK>(w, sr, si, first_id + env);
-  env_step<real, NJ, TK>(w, m, actions + (size_t)env * NU, seed, max_traj_len, autoreset, 0, 1, obs + (size_t)env * W::NOBS,
+  env_step<real, NJ, TK, STAIRS>(w, m, actions + (size_t)env * NU, seed, max_traj_len, autoreset, 0, 1, obs + (size_t)env * W::NOBS,
                      term_obs ? term_obs + (size_t)env * W::NOBS : nullptr, reward + env,
                      rew_terms ? rew_terms + (size_t)env * NREW : nullptr, done + env, ended + env,
-                     ep_len ? ep_len + env : nullptr, ep_rew ? ep_rew + env : nullptr);
+                     ep_len ? ep_len + env : nullptr, ep_rew ? ep_rew + env : nullptr, STAIRS ? level + env : nullptr, n_levels);
   store_state<real, NJ, TK>(w, sr, si);
 }
 
 // the shipped carving: W warps per block (one env each), a __syncthreads() per substep so the warps of an SM share
-// instruction-cache fills (far fewer no-instruction stalls); W from LHW_WARPS_PER_BLOCK or the defaults below
-template <class real, int NJ, int TK>
+// instruction-cache fills (far fewer no-instruction stalls); W from LHW_WARPS_PER_BLOCK or the defaults below.  STAIRS: as step_kernel
+template <class real, int NJ, int TK, bool STAIRS = false>
 // LHW_X_REGCAP (candidate, tools/ab_variants.py): the register budget of the fp64 lock-step kernel as "threads per SM" — 512 = 127
 // registers (16 warps per SM, the shipped kernel), 576 = 112 (18 warps), 640 = 96 (20 warps)
 #ifndef LHW_X_REGCAP
@@ -161,7 +167,7 @@ __global__ void __launch_bounds__(sizeof(real) == 8 ? LHW_X_REGCAP : 896, 1)
                    const real* __restrict__ actions, int max_traj_len, int autoreset, real* __restrict__ obs,
                    real* __restrict__ term_obs, real* __restrict__ reward, real* __restrict__ rew_terms,
                    int32_t* __restrict__ done, int32_t* __restrict__ ended, int32_t* __restrict__ ep_len,
-                   real* __restrict__ ep_rew, int sync_mode) {
+                   real* __restrict__ ep_rew, int sync_mode, int32_t* __restrict__ level = nullptr, int n_levels = 0) {
   using W = Work<real, NJ, TK>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5;
@@ -174,10 +180,10 @@ __global__ void __launch_bounds__(sizeof(real) == 8 ? LHW_X_REGCAP : 896, 1)
   real* sr = state_r + (size_t)e * NR;
   int32_t* si = state_i + (size_t)e * NSTATE_I;
   if (alive) load_state<real, NJ, TK>(w, sr, si, first_id + e);
-  env_step<real, NJ, TK>(w, m, actions + (size_t)e * NU, seed, max_traj_len, autoreset, sync_mode, alive, obs + (size_t)e * W::NOBS,
+  env_step<real, NJ, TK, STAIRS>(w, m, actions + (size_t)e * NU, seed, max_traj_len, autoreset, sync_mode, alive, obs + (size_t)e * W::NOBS,
                      term_obs ? term_obs + (size_t)e * W::NOBS : nullptr, reward + e,
                      rew_terms ? rew_terms + (size_t)e * NREW : nullptr, done + e, ended + e,
-                     ep_len ? ep_len + e : nullptr, ep_rew ? ep_rew + e : nullptr);
+                     ep_len ? ep_len + e : nullptr, ep_rew ? ep_rew + e : nullptr, STAIRS ? level + e : nullptr, n_levels);
   if (alive) store_state<real, NJ, TK>(w, sr, si);
 }
 
@@ -252,6 +258,12 @@ struct lhw_sim {
   virtual int footstep_limits(int* nplan, double* max_height) const = 0;
   virtual void reset_footsteps(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mode,
                                const void* value, int fresh, void* obs, cudaStream_t st) = 0;
+  virtual int stairs_refusal() const = 0;
+  virtual void reset_stairs(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
+                            int fresh, void* obs, const int32_t* level, int n_levels, cudaStream_t st) = 0;
+  virtual void step_stairs(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
+                           int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
+                           int32_t* ended, int32_t* ep_len, void* ep_rew, int32_t* level, int n_levels, cudaStream_t st) = 0;
   virtual void set_step_height(double h) = 0;
 };
 
@@ -277,8 +289,13 @@ template <class real, int NJ, int TK> int prepare_variant(lhw_sim* s) {
   if (prepare_kernel(step_kernel<real, NJ, TK>, s->work_bytes) || prepare_kernel(reset_kernel<real, NJ, TK>, s->work_bytes)) return -10;
   if constexpr (Cfg<NJ, TK>::STEP) {
     if (prepare_kernel(reset_kernel<real, NJ, TK, true>, s->work_bytes)) return -10;
+    if (prepare_kernel(reset_kernel<real, NJ, TK, false, true>, s->work_bytes) || prepare_kernel(step_kernel<real, NJ, TK, true>, s->work_bytes))
+      return -10;
   }
   if (s->warps_per_block > 1 && prepare_kernel(step_kernel_mw<real, NJ, TK>, s->work_bytes * s->warps_per_block)) return -10;
+  if constexpr (Cfg<NJ, TK>::STEP) {
+    if (s->warps_per_block > 1 && prepare_kernel(step_kernel_mw<real, NJ, TK, true>, s->work_bytes * s->warps_per_block)) return -10;
+  }
   return 0;
 }
 
@@ -406,6 +423,39 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
     if constexpr (Cfg<NJ, TK>::STEP)
       reset_kernel<real, NJ, TK, true><<<n_envs, 32, work_bytes, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, nullptr,
                                                                        fresh, (real*)obs, mode, (const real*)value);
+  }
+
+  int stairs_refusal() const override {
+    if constexpr (Cfg<NJ, TK>::STEP) return 0;
+    else
+      return fail(-2, std::string(NJ == 5 ? (TK == 3 ? "h1_walk" : "h1") : TK == 2 ? "jvrc_walk_terrain" : "jvrc_walk") +
+                          " has no stair curriculum: only jvrc_step (SteppingTask) takes one");
+  }
+
+  void reset_stairs(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask, int fresh,
+                    void* obs, const int32_t* level, int n_levels, cudaStream_t st) override {
+    if constexpr (Cfg<NJ, TK>::STEP)
+      reset_kernel<real, NJ, TK, false, true><<<n_envs, 32, work_bytes, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id, mask,
+                                                                              fresh, (real*)obs, nullptr, nullptr, level, n_levels);
+  }
+
+  void step_stairs(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
+                   int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
+                   int32_t* ended, int32_t* ep_len, void* ep_rew, int32_t* level, int n_levels, cudaStream_t st) override {
+    if constexpr (Cfg<NJ, TK>::STEP) {
+      const int wpb = warps_per_block, grid = (n_envs + wpb - 1) / wpb;
+      const size_t smem = work_bytes * wpb;
+      if (wpb > 1)
+        step_kernel_mw<real, NJ, TK, true><<<grid, wpb * 32, smem, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id,
+                                                                         (const real*)actions, max_traj_len, autoreset, (real*)obs,
+                                                                         (real*)term_obs, (real*)reward, (real*)rew_terms, done, ended,
+                                                                         ep_len, (real*)ep_rew, sync_mode, level, n_levels);
+      else
+        step_kernel<real, NJ, TK, true><<<grid, 32, smem, st>>>((real*)state_r, state_i, n_envs, seed, first_env_id,
+                                                                (const real*)actions, max_traj_len, autoreset, (real*)obs, (real*)term_obs,
+                                                                (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew,
+                                                                level, n_levels);
+    }
   }
 
   void set_step_height(double h) override {
@@ -563,6 +613,42 @@ int lhw_sim_reset_footsteps(lhw_sim* s, void* state_r, int32_t* state_i, int n_e
   cudaStream_t st = (cudaStream_t)stream;
   if (s->bind(st)) return -10;
   s->reset_footsteps(state_r, state_i, n_envs, seed, first_env_id, mode, value, fresh, obs, st);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+static int check_stairs(const lhw_sim* s, int n_levels, const char* what) {
+  if (const int rc = s->stairs_refusal()) return fail(rc, std::string(what) + ": " + g_err);
+  if (n_levels < 2 || n_levels > STAIR_MAX_LEVELS)
+    return fail(-2, std::string(what) + ": n_levels must lie in 2.." + std::to_string(STAIR_MAX_LEVELS) + ", got " + std::to_string(n_levels));
+  return 0;
+}
+
+int lhw_sim_reset_stairs(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                         const int32_t* mask, int fresh, void* obs, const int32_t* level, int n_levels, void* stream) {
+  if (!s || !state_r || !state_i || !level) return fail(-1, "null argument");
+  if (const int rc = check_stairs(s, n_levels, "lhw_sim_reset_stairs")) return rc;
+  if (n_envs <= 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (s->bind(st)) return -10;
+  s->reset_stairs(state_r, state_i, n_envs, seed, first_env_id, mask, fresh, obs, level, n_levels, st);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_step_stairs(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                        const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
+                        void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, int32_t* level, int n_levels,
+                        void* stream) {
+  if (!s || !state_r || !state_i || !actions || !obs || !reward || !done || !ended || !level) return fail(-1, "null argument");
+  if (const int rc = check_stairs(s, n_levels, "lhw_sim_step_stairs")) return rc;
+  if (n_envs <= 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (s->bind(st)) return -10;
+  s->step_stairs(state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs, term_obs, reward, rew_terms,
+                 done, ended, ep_len, ep_rew, level, n_levels, st);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .sim_step_stairs, .sim_reset_stairs, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -47,23 +47,27 @@ SimInfo sim_info(int64_t handle) {
           lhw_sim_obs_dim(s), lhw_sim_act_dim(s)};
 }
 
-void sim_reset(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const OptTensor& mask, bool fresh,
-               Tensor obs) {
-  const SimInfo I = sim_info(sim);
+void check_reset(const SimInfo& I, const Tensor& state_r, const Tensor& state_i, const OptTensor& mask, const Tensor& obs) {
   const int64_t n = state_r.size(0);
   check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
   check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
   check_cuda(obs, "obs", I.real, I.device); check_shape(obs, "obs", {n, I.nobs});
   if (mask) { check_cuda(*mask, "mask", at::kInt, I.device); check_shape(*mask, "mask", {n}); }
+}
+
+void sim_reset(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const OptTensor& mask, bool fresh,
+               Tensor obs) {
+  const SimInfo I = sim_info(sim);
+  const int64_t n = state_r.size(0);
+  check_reset(I, state_r, state_i, mask, obs);
   c10::cuda::CUDAGuard guard(I.device);
   ok(lhw_sim_reset(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
                    mask ? mask->data_ptr<int32_t>() : nullptr, fresh ? 1 : 0, obs.data_ptr(), stream_of(state_r)), "lhw_sim_reset");
 }
 
-void sim_step(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const Tensor& actions,
-              int64_t max_traj_len, bool autoreset, Tensor obs, const OptTensor& term_obs, Tensor reward, const OptTensor& rew_terms,
-              Tensor done, Tensor ended, const OptTensor& ep_len, const OptTensor& ep_rew) {
-  const SimInfo I = sim_info(sim);
+void check_step(const SimInfo& I, const Tensor& state_r, const Tensor& state_i, const Tensor& actions, int64_t max_traj_len, const Tensor& obs,
+                const OptTensor& term_obs, const Tensor& reward, const OptTensor& rew_terms, const Tensor& done, const Tensor& ended,
+                const OptTensor& ep_len, const OptTensor& ep_rew) {
   const int64_t n = state_r.size(0);
   check_cuda(state_r, "state_r", I.real, I.device); check_shape(state_r, "state_r", {n, I.nr});
   check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
@@ -77,6 +81,14 @@ void sim_step(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t
   if (ep_len) { check_cuda(*ep_len, "ep_len", at::kInt, I.device); check_shape(*ep_len, "ep_len", {n}); }
   if (ep_rew) { check_cuda(*ep_rew, "ep_rew", I.real, I.device); check_shape(*ep_rew, "ep_rew", {n}); }
   TORCH_CHECK(max_traj_len > 0, "lhw: max_traj_len must be positive");
+}
+
+void sim_step(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const Tensor& actions,
+              int64_t max_traj_len, bool autoreset, Tensor obs, const OptTensor& term_obs, Tensor reward, const OptTensor& rew_terms,
+              Tensor done, Tensor ended, const OptTensor& ep_len, const OptTensor& ep_rew) {
+  const SimInfo I = sim_info(sim);
+  const int64_t n = state_r.size(0);
+  check_step(I, state_r, state_i, actions, max_traj_len, obs, term_obs, reward, rew_terms, done, ended, ep_len, ep_rew);
   c10::cuda::CUDAGuard guard(I.device);
   ok(lhw_sim_step(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
                   actions.data_ptr(), (int)max_traj_len, autoreset ? 1 : 0, obs.data_ptr(), term_obs ? term_obs->data_ptr() : nullptr,
@@ -200,6 +212,44 @@ void sim_reset_footsteps(int64_t sim, Tensor state_r, Tensor state_i, int64_t se
   ok(lhw_sim_reset_footsteps(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
                              mode.data_ptr<int32_t>(), value.data_ptr(), fresh ? 1 : 0, obs.data_ptr(), stream_of(state_r)),
      "lhw_sim_reset_footsteps");
+}
+
+// the stair curriculum's level tensor [n] int32 and its level count (lhw_sim_step_stairs / lhw_sim_reset_stairs, DESIGN.md §7.8);
+// a variant without the curriculum is named by the C-ABI's refusal
+void check_stairs(const SimInfo& I, const Tensor& level, int64_t n, int64_t n_levels) {
+  check_cuda(level, "level", at::kInt, I.device); check_shape(level, "level", {n});
+  TORCH_CHECK(n_levels >= 2 && n_levels <= 21, "lhw: n_levels must lie in 2..21, got ", n_levels);
+}
+
+void sim_step_stairs(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const Tensor& actions,
+                     int64_t max_traj_len, bool autoreset, Tensor obs, const OptTensor& term_obs, Tensor reward, const OptTensor& rew_terms,
+                     Tensor done, Tensor ended, const OptTensor& ep_len, const OptTensor& ep_rew, Tensor level, int64_t n_levels) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_step(I, state_r, state_i, actions, max_traj_len, obs, term_obs, reward, rew_terms, done, ended, ep_len, ep_rew);
+  check_stairs(I, level, n, n_levels);
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_step_stairs(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                         actions.data_ptr(), (int)max_traj_len, autoreset ? 1 : 0, obs.data_ptr(), term_obs ? term_obs->data_ptr() : nullptr,
+                         reward.data_ptr(), rew_terms ? rew_terms->data_ptr() : nullptr, done.data_ptr<int32_t>(), ended.data_ptr<int32_t>(),
+                         ep_len ? ep_len->data_ptr<int32_t>() : nullptr, ep_rew ? ep_rew->data_ptr() : nullptr, level.data_ptr<int32_t>(),
+                         (int)n_levels, stream_of(state_r)),
+     "lhw_sim_step_stairs");
+}
+
+void sim_reset_stairs(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const OptTensor& mask, bool fresh,
+                      Tensor obs, const Tensor& level, int64_t n_levels) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_reset(I, state_r, state_i, mask, obs);
+  check_stairs(I, level, n, n_levels);
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_reset_stairs(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                          mask ? mask->data_ptr<int32_t>() : nullptr, fresh ? 1 : 0, obs.data_ptr(), level.data_ptr<int32_t>(),
+                          (int)n_levels, stream_of(state_r)),
+     "lhw_sim_reset_stairs");
 }
 
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
@@ -409,6 +459,11 @@ TORCH_LIBRARY(lhw, m) {
   m.def("sim_command_accumulate(int sim, Tensor state_r, Tensor done, Tensor(a!) acc) -> ()");
   m.def("sim_reset_footsteps(int sim, Tensor(a!) state_r, Tensor(b!) state_i, int seed, int first_env_id, Tensor mode, Tensor value, "
         "bool fresh, Tensor(c!) obs) -> ()");
+  m.def("sim_step_stairs(int sim, Tensor(a!) state_r, Tensor(b!) state_i, int seed, int first_env_id, Tensor actions, int max_traj_len, "
+        "bool autoreset, Tensor(c!) obs, Tensor(d!)? term_obs, Tensor(e!) reward, Tensor(f!)? rew_terms, Tensor(g!) done, Tensor(h!) ended, "
+        "Tensor(i!)? ep_len, Tensor(j!)? ep_rew, Tensor(k!) level, int n_levels) -> ()");
+  m.def("sim_reset_stairs(int sim, Tensor(a!) state_r, Tensor(b!) state_i, int seed, int first_env_id, Tensor? mask, bool fresh, "
+        "Tensor(c!) obs, Tensor level, int n_levels) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -443,6 +498,8 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_set_command", &sim_set_command);
   m.impl("sim_command_accumulate", &sim_command_accumulate);
   m.impl("sim_reset_footsteps", &sim_reset_footsteps);
+  m.impl("sim_step_stairs", &sim_step_stairs);
+  m.impl("sim_reset_stairs", &sim_reset_stairs);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

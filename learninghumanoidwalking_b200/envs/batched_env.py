@@ -31,6 +31,8 @@ MODE_HELD = 1 << 30
 # chosen footstep plans (reset_footsteps, DESIGN.md §7.7): the SteppingTask's plan types in the order of the kernel's mode word
 # (csrc/sim_core.h ST_*)
 FOOTSTEP_MODES = ("CURVED", "STANDING", "BACKWARD", "LATERAL", "FORWARD")
+# the stair curriculum (stair_curriculum=H, DESIGN.md §7.8): levels of 0.01 m up to H <= 0.2 m (csrc/sim_core.h STAIR_MAX_LEVELS)
+STAIR_STEP, STAIR_MAX_HEIGHT = 0.01, 0.2
 N_REWARD_SLOTS = 10   # width of the kernel's reward-term record (csrc/sim_core.h NREW); unused slots are 0
 # h1_walk (DESIGN.md §4.6): joints (hip_yaw, hip_roll, hip_pitch, knee, ankle), left leg then right.  The mirror swaps the legs and
 # negates yaw and roll; in the observation also the root roll and the x, z angular velocities.  The 8 walking-task words map to
@@ -54,6 +56,23 @@ def push_interval_steps(push_vel: float, push_interval: float, dt: float) -> int
     return int(round(push_interval / dt))
 
 
+def stair_levels(model: str, stair_curriculum: float) -> int:
+    """The number of levels K = H / 0.01 + 1 of a stair curriculum up to H = stair_curriculum m, or 0 when H is 0 (off), after
+    refusing a model other than jvrc_step and an H that is not finite, negative, above 0.2 or not a multiple of 0.01
+    (DESIGN.md §7.8)."""
+    h = float(stair_curriculum)
+    if not np.isfinite(h) or h < 0 or h > STAIR_MAX_HEIGHT:
+        raise ValueError(f"stair_curriculum must be a stair height in (0, {STAIR_MAX_HEIGHT:g}] m, or 0 (off), got {stair_curriculum}")
+    if h == 0:
+        return 0
+    k = round(h / STAIR_STEP)
+    if abs(k * STAIR_STEP - h) > 1e-9:
+        raise ValueError(f"stair_curriculum must be a multiple of {STAIR_STEP:g} m, got {stair_curriculum}")
+    if model != "jvrc_step":
+        raise ValueError(f"{model} has no stair curriculum: only jvrc_step (SteppingTask) takes one")
+    return k + 1
+
+
 class _Robot(SimpleNamespace):
     """The attributes the trainer reads / writes on `env.robot` (robots/robot_base.py:35, run_experiment.py:123-125).
     Writing `iteration_count` (rl/workers/rollout_worker.py:95) drives the SteppingTask's height curriculum."""
@@ -69,7 +88,12 @@ class BatchedHumanoidEnv:
                  first_env_id: int = 0, device: int | torch.device | None = None, max_traj_len: int = 400,
                  tolerance: float | None = None, max_iter: int | None = None, observation_noise: bool = True,
                  domain_randomization: bool = True, init_noise: bool = True, pd_gain_randomization: float = 0.0,
-                 iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0):
+                 iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0,
+                 stair_curriculum: float = 0.0):
+        # a stair level per env (DESIGN.md §7.8): every reset builds a FORWARD plan with its level's stair height, and each
+        # auto-reset first moves the level by the ending FORWARD episode; off at 0, and then the launches are the plain ones
+        self.stair_levels = stair_levels(model, stair_curriculum)
+        self.stair_curriculum = float(stair_curriculum) if self.stair_levels else 0.0
         if not torch.cuda.is_available():
             raise _lib.LhwError("BatchedHumanoidEnv needs a CUDA device (no CPU fallback on the rollout path)")
         if device is None:
@@ -111,6 +135,8 @@ class BatchedHumanoidEnv:
         self.ep_len = torch.zeros(n, dtype=torch.int32, device=dev)
         self.ep_rew = torch.zeros(n, dtype=self.dtype, device=dev)
         self._fresh = True
+        # int32 [N]: each env's stair level in [0, stair_levels); None without the curriculum
+        self.stair_level = torch.zeros(n, dtype=torch.int32, device=dev) if self.stair_levels else None
         # ---- reference-facing attributes (envs/jvrc/jvrc_base.py:69-131, envs/jvrc/jvrc_walk.py:43-63)
         cfg = self.mj["cfg"]
         self.history_len = cfg["obs_history_len"]
@@ -178,7 +204,10 @@ class BatchedHumanoidEnv:
         L = _lib.lib()
         if mask is not None:
             mask = mask.to(device=self.device, dtype=torch.int32).contiguous()
-        if _lib.use_torch_ops():
+        if self.stair_level is not None:
+            _lib.ops().sim_reset_stairs(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, mask,
+                                        bool(self._fresh and mask is None), self.obs, self.stair_level, self.stair_levels)
+        elif _lib.use_torch_ops():
             _lib.ops().sim_reset(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, mask,
                                  bool(self._fresh and mask is None), self.obs)
         else:
@@ -195,6 +224,12 @@ class BatchedHumanoidEnv:
         With autoreset the RolloutWorker semantics apply (see include/lhw_b200.h: lhw_sim_step)."""
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
+        if self.stair_level is not None:
+            _lib.ops().sim_step_stairs(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, actions, self.max_traj_len,
+                                       bool(autoreset), self.obs, self.term_obs, self.reward, self.rew_terms, self.done, self.ended,
+                                       self.ep_len, self.ep_rew, self.stair_level, self.stair_levels)
+            self._push_random(0, self.num_envs)
+            return self.obs, self.reward, self.done, self.ended
         if _lib.use_torch_ops():     # torch.ops.lhw.sim_step: device / dtype / shape checks, then the C-ABI launch
             _lib.ops().sim_step(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, actions, self.max_traj_len,
                                 bool(autoreset), self.obs, self.term_obs, self.reward, self.rew_terms, self.done, self.ended,
@@ -221,6 +256,12 @@ class BatchedHumanoidEnv:
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
         out = (self.obs[sl], self.reward[sl], self.done[sl], self.ended[sl])
+        if self.stair_level is not None:
+            _lib.ops().sim_step_stairs(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
+                                       self.max_traj_len, bool(autoreset), out[0], self.term_obs[sl], out[1], self.rew_terms[sl], out[2],
+                                       out[3], self.ep_len[sl], self.ep_rew[sl], self.stair_level[sl], self.stair_levels)
+            self._push_random(lo, hi)
+            return out
         if _lib.use_torch_ops():
             _lib.ops().sim_step(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
                                 self.max_traj_len, bool(autoreset), out[0], self.term_obs[sl], out[1], self.rew_terms[sl], out[2], out[3],

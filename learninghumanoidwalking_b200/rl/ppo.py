@@ -203,7 +203,8 @@ class PPO:
         return dict(format=snapshot.FORMAT, itr=int(itr), rank=self.rank, world=self.world, first_env_id=env.first_env_id,
                     num_envs=env.num_envs, model=env.model_name, precision=env.precision, seed=env.seed,
                     state_r=env.state_r.cpu(), state_i=env.state_i.cpu(), fresh=bool(env._fresh),
-                    worker=self.workers[0].state_dict(), cpu_rng=torch.get_rng_state())
+                    worker=self.workers[0].state_dict(), cpu_rng=torch.get_rng_state(),
+                    **({} if getattr(env, "stair_level", None) is None else dict(stair_level=env.stair_level.cpu())))
 
     def restore(self, run_dir) -> int:
         """Load the last complete snapshot of `run_dir` into this freshly built PPO and its environment and return the iteration
@@ -226,6 +227,13 @@ class PPO:
             if have.shape != want.shape or have.dtype != want.dtype:
                 raise SnapshotError(f"{name} of the snapshot is {tuple(have.shape)} {have.dtype}, this run has "
                                     f"{tuple(want.shape)} {want.dtype}")
+        stair_level = getattr(env, "stair_level", None)
+        if stair_level is not None:
+            if "stair_level" not in shard:
+                raise SnapshotError("the snapshot holds no stair levels (was it written by a run without --stair-curriculum?)")
+            if shard["stair_level"].shape != stair_level.shape or shard["stair_level"].dtype != stair_level.dtype:
+                raise SnapshotError(f"stair_level of the snapshot is {tuple(shard['stair_level'].shape)} {shard['stair_level'].dtype}, "
+                                    f"this run has {tuple(stair_level.shape)} {stair_level.dtype}")
         with torch.no_grad():
             self._flat_param.copy_(learner["flat_param"])
             self._flat_m.copy_(learner["exp_avg"])
@@ -235,6 +243,8 @@ class PPO:
                 getattr(getattr(self, net), name).copy_(v)
             env.state_r.copy_(shard["state_r"])
             env.state_i.copy_(shard["state_i"])
+            if stair_level is not None:
+                stair_level.copy_(shard["stair_level"])
         env._fresh = bool(shard["fresh"])
         a_opt.step_count, c_opt.step_count = learner["step_count"]
         if getattr(self, "schedule", "fixed") == "adaptive":
@@ -588,6 +598,7 @@ class PPO:
                 self._comm.status()    # raises if a peer missed a gradient exchange (bounded spin in the kernels)
             adaptive = getattr(self, "schedule", "fixed") == "adaptive"
             lr_now = self._comm.get_lr() if adaptive else None     # the stream has just been synchronised
+            stairs = self._stair_stats()     # (mean stair height, fraction at the top level) or None
             optimize_time = time.time() - t1
             total_time = time.time() - train_start
             fps = self.total_steps / total_time
@@ -598,6 +609,8 @@ class PPO:
                             clip_frac=stats[6]))
             if adaptive:
                 log[-1]["lr"] = lr_now
+            if stairs is not None:
+                log[-1].update(mean_stair_height=stairs[0], top_stair_fraction=stairs[1])
             if verbose and self.rank == 0:
                 print(f"Optimizer took: {optimize_time:.2f}s")
                 print("-" * 37)
@@ -605,7 +618,8 @@ class PPO:
                              ("Mirror loss", stats[4]), ("Imitation loss", stats[5]), ("Mean KL Div", stats[3]),
                              ("Mean Entropy", stats[1]), ("Clip Fraction", stats[6]),
                              ("Mean noise std", float(torch.as_tensor(self.policy.stds).mean())),
-                             *((("Learning rate", lr_now),) if adaptive else ())):
+                             *((("Learning rate", lr_now),) if adaptive else ()),
+                             *((("Mean stair height", stairs[0]), ("Top stair level", stairs[1])) if stairs is not None else ())):
                     print(f"| {k:>15} | {v:>15.5g} |")
                 print("-" * 37)
                 eta = round((n_itr - itr) * total_time / (itr + 1))
@@ -616,7 +630,9 @@ class PPO:
                                ("Loss/imitation", stats[5]), ("Train/mean_reward", ep_rew), ("Train/mean_episode_length", ep_len),
                                ("Train/mean_noise_std", float(torch.as_tensor(self.policy.stds).mean())), ("Time/fps", fps),
                                ("Time/sample_time", sample_time), ("Time/optimize_time", optimize_time),
-                               ("Time/total_elapsed", total_time), *((("Train/learning_rate", lr_now),) if adaptive else ())):
+                               ("Time/total_elapsed", total_time), *((("Train/learning_rate", lr_now),) if adaptive else ()),
+                               *((("Train/mean_stair_height", stairs[0]), ("Train/top_stair_fraction", stairs[1]))
+                                 if stairs is not None else ())):
                     writer.add_scalar(tag, v, itr)
             if (itr == 0 and getattr(self, "eval_at_start", True)) or (itr + 1) % self.eval_freq == 0:     # rl/algos/ppo.py:597-615
                 t2 = time.time()
@@ -637,6 +653,22 @@ class PPO:
             writer.flush()
             writer.close()
         return log
+
+    def _stair_stats(self):
+        """The stair curriculum's state over every env of every rank (DESIGN.md §7.8): (mean of 0.01 L, fraction of envs at the
+        top level K - 1), or None without the curriculum.  One small copy to the host, after the iteration's host sync."""
+        env = self._inner_env()
+        level = getattr(env, "stair_level", None)
+        if level is None:
+            return None
+        top = env.stair_levels - 1
+        lv = level.clamp(0, top)   # as the kernels read it
+        t = torch.stack([lv.sum(dtype=torch.float64), (lv == top).sum(dtype=torch.float64),
+                         torch.tensor(float(lv.numel()), dtype=torch.float64, device=lv.device)])
+        if self.world > 1:
+            dist.all_reduce(t, op=dist.ReduceOp.SUM)
+        s, n_top, n = t.tolist()
+        return 0.01 * s / n, n_top / n
 
     def _tensorboard_writer(self, purge_step=None):
         """TrainingLogger (rl/utils/logger.py:24-45): a SummaryWriter on the run directory; None if tensorboard is absent

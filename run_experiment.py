@@ -28,7 +28,10 @@ run prints the achieved velocities and tracking errors of each cell; without it,
 (and its video) and re-applied after every reset there.  `eval --footsteps forward:0,0.05,0.1 lateral:left,right backward curved
 standing` chooses jvrc_step's stepping-stone plans (DESIGN §7.7): with --num-envs N env i resets with the plan of cell i mod C and the
 run prints the falls and footsteps reached of each cell; without it, the one plan is chosen at every reset of the single-env
-roll-out (and its video).
+roll-out (and its video).  `train --env jvrc_step --stair-curriculum H` gives every env a stair level (DESIGN §7.8): its FORWARD
+plans climb or descend stairs of 0.01 L m, and L goes up by one after a FORWARD episode that did not fall and reached half its
+footsteps, and down by one after one that fell short of half, between 0 and H; the iteration table and TensorBoard show the mean
+stair height and the fraction of envs at the top level.
 """
 import argparse
 import os
@@ -73,6 +76,8 @@ TRAIN_FLAGS = [
     ("--desired-kl", dict(type=_F, default=0.01, help="target KL of --schedule adaptive")),
     ("--push-vel", dict(type=_F, default=0.0, help="random root-velocity pushes of up to V m/s per horizontal axis (0: off; DESIGN §7.5)")),
     ("--push-interval", dict(type=_F, default=15.0, help="mean seconds between two random pushes of an env")),
+    ("--stair-curriculum", dict(type=_F, default=0.0, help="jvrc_step: a stair level per env up to H m, a multiple of 0.01 in (0, 0.2], "
+                                                           "moved by each FORWARD episode (0: off, the reference's schedule; DESIGN §7.8)")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -120,6 +125,9 @@ def print_system_info(args, training=True):
         push_vel = getattr(args, "push_vel", 0.0)
         print(f"Random pushes: up to {push_vel} m/s about every {getattr(args, 'push_interval', 15.0)} s" if push_vel > 0
               else "Random pushes: off")
+        stairs = getattr(args, "stair_curriculum", 0.0)
+        if stairs:
+            print(f"Stair curriculum: levels of 0.01 m up to {stairs} m")
     print("=" * 60)
 
 
@@ -167,7 +175,8 @@ def make_env_fn(args, rank, world, local):
     seed = args.seed if args.seed is not None else 0
     env_fn = partial(Env, n_local, precision=args.precision, seed=seed, first_env_id=first, device=local,
                      max_traj_len=args.max_traj_len, path_to_yaml=args.yaml, push_vel=getattr(args, "push_vel", 0.0),
-                     push_interval=getattr(args, "push_interval", 15.0))   # an experiment.pkl without them: no pushes
+                     push_interval=getattr(args, "push_interval", 15.0),   # an experiment.pkl without them: no pushes
+                     stair_curriculum=getattr(args, "stair_curriculum", 0.0))   # nor a stair curriculum
     _env = env_fn()
     if not args.no_mirror:
         try:
@@ -211,9 +220,21 @@ def check_push(args):
         raise SystemExit(f"train --push-vel {push_vel} --push-interval {push_interval}: {e}")
 
 
+def check_stairs(args):
+    """Refuse a stair curriculum the env would refuse, before any environment or run directory exists."""
+    from learninghumanoidwalking_b200.envs.batched_env import stair_levels
+    stairs = getattr(args, "stair_curriculum", 0.0)
+    import_env(args.env)
+    try:
+        stair_levels(args.env, stairs)
+    except ValueError as e:
+        raise SystemExit(f"train --stair-curriculum {stairs}: {e}")
+
+
 def run_experiment(args):
     from learninghumanoidwalking_b200.rl import PPO
     check_push(args)
+    check_stairs(args)
     rank, world, local = _dist_setup()
     timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
     args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
