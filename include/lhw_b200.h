@@ -157,6 +157,24 @@ int lhw_sim_step_stairs(lhw_sim* sim, void* state_r, int32_t* state_i, int n_env
                         void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, int32_t* level, int n_levels,
                         void* stream);
 
+/* lhw_sim_step_delay: lhw_sim_step with an action delay per env (DESIGN.md §7.9), every variant.  delay [n] (device int32) holds
+ * each env's delay d in physics substeps, clamped to [0, frame_skip] where it is read, once per control step.  In the control
+ * step, substeps 0 .. d-1 drive the PD loop towards the previous control step's target, substeps d .. frame_skip-1 towards this
+ * step's; nothing else changes (smoothing, gains, rewards, observations, termination, auto-reset).  The first step of an episode
+ * has no previous target and so is never delayed.  d = 0 is lhw_sim_step bit for bit; d = frame_skip delays the action by one
+ * whole control step.  level != NULL (jvrc_step only) adds the stair curriculum of lhw_sim_step_stairs, with its refusals.
+ * Nothing writes delay.
+ * lhw_sim_draw_delay: the random delays.  Every env whose mask [n] word is non-zero (every env when mask is NULL; pass the step's
+ * `ended`, or a reset's mask) gets delay[i] = randint(u[0], max_delay + 1) with u = philox(seed, first_env_id + i, rng_ctr,
+ * 71), rng_ctr the record's event counter (state_i[i][4]) as the reset left it.  Only delay is written; max_delay outside
+ * 0..frame_skip is refused with -2.  Reads no model constants. */
+int lhw_sim_step_delay(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                       const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
+                       void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, const int32_t* delay,
+                       int32_t* level, int n_levels, void* stream);
+int lhw_sim_draw_delay(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
+                       int max_delay, int32_t* delay, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

@@ -2238,14 +2238,20 @@ struct StepOut {
   int32_t* done; int32_t* ended; int32_t* ep_len; void* ep_rew;
 };
 
+// the action delay (lhw_sim_step_delay, DESIGN.md §7.9): an env's delay in physics substeps, clamped to [0, frame_skip] where it
+// is read
+LHW_DEV int action_delay_clamp(int d, int frame_skip) { return d < 0 ? 0 : d > frame_skip ? frame_skip : d; }
+
 // BaseHumanoidEnv.step + the RolloutWorker's bookkeeping (traj_len truncation, auto-reset, episode stats).  STAIRS (SteppingTask
 // only, DESIGN.md §7.8): *level is the env's stair-curriculum level of n_levels; an auto-reset first moves it by the ending episode
-// when that was a FORWARD one (stair_level_next), then resets with its stair height
-template <class real, int NJ, int TK, bool STAIRS = false>
+// when that was a FORWARD one (stair_level_next), then resets with its stair height.  DELAY (DESIGN.md §7.9): substeps
+// 0 .. delay-1 drive the PD loop towards the previous control step's target (prev_action, which holds it until the record update
+// below), the rest towards this step's; delay is already clamped to [0, frame_skip].  At delay 0 the step is the plain one
+template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false>
 LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const real* action, uint32_t seed, int max_traj_len,
                       int autoreset, const int block_sync, const int alive, real* obs_out, real* term_obs_out, real* reward_out, real* rew_terms_out,
                       int32_t* done_out, int32_t* ended_out, int32_t* ep_len_out, real* ep_rew_out, int32_t* level = nullptr,
-                      int n_levels = 0) {
+                      int n_levels = 0, const int delay = 0) {
   constexpr int NU = 2 * NJ, NOBS = Work<real, NJ, TK>::NOBS;
   // action smoothing + nominal offsets (base_humanoid_env.py:209-212, robot_base.py:80-85)
   // one event counter per control step: every draw of this step is keyed by rng_ctr + 1 (stored below)
@@ -2271,7 +2277,14 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
   LHW_SYNC();
   for (int sidx = 0; sidx < m.frame_skip; sidx++) {
     LHW_LANES(l) {
-      if (l < NU) w.ctrl[l] = w.kp_step[l] * (w.target[l] - w.act_len[l]) + w.kd_step[l] * ((real)0 - w.act_vel[l]);
+      if constexpr (DELAY) {
+        if (l < NU) {
+          const real tg = sidx < delay ? w.prev_action[l] : w.target[l];
+          w.ctrl[l] = w.kp_step[l] * (tg - w.act_len[l]) + w.kd_step[l] * ((real)0 - w.act_vel[l]);
+        }
+      } else {
+        if (l < NU) w.ctrl[l] = w.kp_step[l] * (w.target[l] - w.act_len[l]) + w.kd_step[l] * ((real)0 - w.act_vel[l]);
+      }
     }
     LHW_SYNC();
     if (alive) substep<real, NJ, TK>(w, m, sidx == m.frame_skip - 1, block_sync, sidx > 0);
@@ -2596,6 +2609,7 @@ LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward,
 // joint velocities are unchanged.  Nothing else of the record is written, and nothing of an env that is not pushed.
 // The random pushes draw on their own Philox stream at the env's event counter, which they only read.  The step and reset
 // bodies above draw on streams 0-5, 8-13, 16-35, 40-48, 50-54 and 60-64, so with pushes off every trajectory is unchanged.
+// The random action delays draw on stream 71 (DELAY_STREAM, delay_draw_env below).
 constexpr uint32_t PUSH_STREAM = 70;
 
 // One env's push; returns 1 when it was pushed.  Explicit mode (d != nullptr): (dx, dy) = (d[0], d[1]), skipped when both are
@@ -2629,6 +2643,19 @@ LHW_DEV int push_env(real* sr, const int32_t* si, uint32_t seed, uint32_t env_id
   sr[A::QVEL + 0] = (real)((double)sr[A::QVEL + 0] + (c * dx - s * dy));
   sr[A::QVEL + 1] = (real)((double)sr[A::QVEL + 1] + (s * dx + c * dy));
   return 1;
+}
+
+// ================================================================= random action delays (lhw_sim_draw_delay, DESIGN.md §7.9)
+// An env that was just reset (sel != 0: its ended word or mask word) draws the delay of its new episode, d ~ U{0 .. max_delay}
+// substeps: randint(u[0], max_delay + 1) with u = philox(seed, env_id, rng_ctr, DELAY_STREAM), at the event counter the reset left
+// (si[4]; every reset increments it).  Only *delay is written.
+constexpr uint32_t DELAY_STREAM = 71;
+
+LHW_DEV void delay_draw_env(const int32_t* si, uint32_t seed, uint32_t env_id, int32_t sel, int max_delay, int32_t* delay) {
+  if (!sel) return;
+  uint32_t u[4];
+  philox(seed, env_id, (uint32_t)si[4], DELAY_STREAM, u);
+  *delay = randint(u[0], max_delay + 1);
 }
 
 // ================================================================= held commands (lhw_sim_set_command, DESIGN.md §7.6)

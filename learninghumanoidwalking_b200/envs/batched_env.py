@@ -73,6 +73,20 @@ def stair_levels(model: str, stair_curriculum: float) -> int:
     return k + 1
 
 
+def action_delay_substeps(seconds, sim_dt: float, control_dt: float) -> np.ndarray:
+    """Action delays in seconds (a number or a sequence) as whole physics substeps (int32 array), after refusing a value that is
+    negative, not finite, above one control step or not a whole number of sim_dt (DESIGN.md §7.9)."""
+    s = np.asarray(seconds, dtype=np.float64).reshape(-1)
+    bad = ~np.isfinite(s) | (s < 0) | (s > control_dt + 1e-12)
+    if bad.any():
+        raise ValueError(f"an action delay must lie in [0, {control_dt:g}] s (one control step), got {s[bad][0]}")
+    k = np.round(s / sim_dt)
+    off = np.abs(k * sim_dt - s) > 1e-9
+    if off.any():
+        raise ValueError(f"an action delay must be a whole number of physics substeps of {sim_dt:g} s, got {s[off][0]}")
+    return k.astype(np.int32)
+
+
 class _Robot(SimpleNamespace):
     """The attributes the trainer reads / writes on `env.robot` (robots/robot_base.py:35, run_experiment.py:123-125).
     Writing `iteration_count` (rl/workers/rollout_worker.py:95) drives the SteppingTask's height curriculum."""
@@ -89,7 +103,7 @@ class BatchedHumanoidEnv:
                  tolerance: float | None = None, max_iter: int | None = None, observation_noise: bool = True,
                  domain_randomization: bool = True, init_noise: bool = True, pd_gain_randomization: float = 0.0,
                  iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0,
-                 stair_curriculum: float = 0.0):
+                 stair_curriculum: float = 0.0, action_delay: float = 0.0):
         # a stair level per env (DESIGN.md §7.8): every reset builds a FORWARD plan with its level's stair height, and each
         # auto-reset first moves the level by the ending FORWARD episode; off at 0, and then the launches are the plain ones
         self.stair_levels = stair_levels(model, stair_curriculum)
@@ -112,6 +126,8 @@ class BatchedHumanoidEnv:
         # random root-velocity pushes after every control step (DESIGN.md §7.5): off at push_vel == 0, and then nothing is launched
         self.push_vel, self.push_interval = float(push_vel), float(push_interval)
         self.push_interval_steps = push_interval_steps(push_vel, push_interval, self.mj["cfg"]["control_dt"])
+        # random action delays (DESIGN.md §7.9): every reset draws its env's delay from U{0 .. action_delay_max} substeps
+        self.action_delay_max = int(action_delay_substeps(action_delay, self.mj["cfg"]["sim_dt"], self.mj["cfg"]["control_dt"])[0])
         if tolerance is None and precision == 32:
             tolerance = 1e-6  # fp32 cannot reach the reference's 1e-10; gradient floor is ~1e-6 of the force scale
         flat = pack_model(self.mj, tolerance=tolerance, max_iter=max_iter, observation_noise=observation_noise,
@@ -137,6 +153,9 @@ class BatchedHumanoidEnv:
         self._fresh = True
         # int32 [N]: each env's stair level in [0, stair_levels); None without the curriculum
         self.stair_level = torch.zeros(n, dtype=torch.int32, device=dev) if self.stair_levels else None
+        # int32 [N]: each env's action delay in physics substeps; None (and the plain step kernels) until random delays or
+        # set_action_delay create it
+        self.action_delay = torch.zeros(n, dtype=torch.int32, device=dev) if self.action_delay_max else None
         # ---- reference-facing attributes (envs/jvrc/jvrc_base.py:69-131, envs/jvrc/jvrc_walk.py:43-63)
         cfg = self.mj["cfg"]
         self.history_len = cfg["obs_history_len"]
@@ -217,6 +236,7 @@ class BatchedHumanoidEnv:
                                            self.obs.data_ptr(), _lib.current_stream_ptr()), "lhw_sim_reset")
         if mask is None:
             self._fresh = False
+        self._draw_delay(0, self.num_envs, mask)
         return self.obs
 
     def step(self, actions: torch.Tensor, autoreset: bool = True):
@@ -224,6 +244,9 @@ class BatchedHumanoidEnv:
         With autoreset the RolloutWorker semantics apply (see include/lhw_b200.h: lhw_sim_step)."""
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
+        if self.action_delay is not None:
+            self._step_delay(0, self.num_envs, actions, autoreset)
+            return self.obs, self.reward, self.done, self.ended
         if self.stair_level is not None:
             _lib.ops().sim_step_stairs(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, actions, self.max_traj_len,
                                        bool(autoreset), self.obs, self.term_obs, self.reward, self.rew_terms, self.done, self.ended,
@@ -256,6 +279,9 @@ class BatchedHumanoidEnv:
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
         out = (self.obs[sl], self.reward[sl], self.done[sl], self.ended[sl])
+        if self.action_delay is not None:
+            self._step_delay(lo, hi, actions, autoreset)
+            return out
         if self.stair_level is not None:
             _lib.ops().sim_step_stairs(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
                                        self.max_traj_len, bool(autoreset), out[0], self.term_obs[sl], out[1], self.rew_terms[sl], out[2],
@@ -278,6 +304,39 @@ class BatchedHumanoidEnv:
                        "lhw_sim_step")
         self._push_random(lo, hi)
         return out
+
+    def _step_delay(self, lo: int, hi: int, actions: torch.Tensor, autoreset: bool) -> None:
+        """The delayed control step of environments [lo, hi) (with the stair curriculum when it is on), then, in random mode and
+        with autoreset, the delay draw of the envs it ended (and so reset), then the random pushes; all on the current stream."""
+        sl = slice(lo, hi)
+        level = None if self.stair_level is None else self.stair_level[sl]
+        _lib.ops().sim_step_delay(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
+                                  self.max_traj_len, bool(autoreset), self.obs[sl], self.term_obs[sl], self.reward[sl], self.rew_terms[sl],
+                                  self.done[sl], self.ended[sl], self.ep_len[sl], self.ep_rew[sl], self.action_delay[sl], level,
+                                  self.stair_levels)
+        if autoreset:
+            self._draw_delay(lo, hi, self.ended[sl])
+        self._push_random(lo, hi)
+
+    def _draw_delay(self, lo: int, hi: int, mask: torch.Tensor | None) -> None:
+        """Random mode: environments [lo, hi) whose mask word is non-zero (all without a mask), just reset, draw their new
+        episode's delay; nothing is launched otherwise (include/lhw_b200.h: lhw_sim_draw_delay)."""
+        if self.action_delay_max:
+            _lib.ops().sim_draw_delay(self._h.value, self.state_i[lo:hi], self.seed, self.first_env_id + lo, mask, self.action_delay_max,
+                                      self.action_delay[lo:hi])
+
+    def set_action_delay(self, seconds) -> None:
+        """Give every environment an action delay: seconds holds N values (a sequence or tensor), each a whole number of physics
+        substeps in [0, control_dt].  In a control step, the first delay / sim_dt substeps still drive the PD loop towards the
+        previous step's target.  The delays hold until each env's next reset draws a new one (random mode, action_delay > 0) or
+        until they are set again (include/lhw_b200.h: lhw_sim_step_delay)."""
+        s = torch.as_tensor(seconds, dtype=torch.float64).detach().to("cpu").reshape(-1)
+        if s.shape != (self.num_envs,):
+            raise ValueError(f"seconds must hold {self.num_envs} numbers, got {tuple(s.shape)}")
+        d = action_delay_substeps(s.numpy(), self.mj["cfg"]["sim_dt"], self.mj["cfg"]["control_dt"])
+        if self.action_delay is None:
+            self.action_delay = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
+        self.action_delay.copy_(torch.from_numpy(d))
 
     def _push_random(self, lo: int, hi: int) -> None:
         """The random pushes of environments [lo, hi) after their control step, on the same stream; none at push_vel == 0.
@@ -355,6 +414,8 @@ class BatchedHumanoidEnv:
                                        mode.to(device=self.device, dtype=torch.int32), value.to(device=self.device, dtype=self.dtype),
                                        self._fresh, self.obs)
         self._fresh = False
+        if self.action_delay_max:
+            self._draw_delay(0, self.num_envs, (mode >= 0).to(device=self.device, dtype=torch.int32))
         return self.obs
 
     def command_accumulate(self, acc: torch.Tensor) -> torch.Tensor:

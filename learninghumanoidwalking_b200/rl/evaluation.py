@@ -18,6 +18,11 @@ body then also launches BatchedHumanoidEnv.command_accumulate, whose per-env rec
 The footstep sweep (`eval --num-envs N --footsteps forward:0,0.05,0.1 lateral:left,right curved standing`, DESIGN.md §7.7, jvrc_step)
 resets env i with the stepping-stone plan of cell i mod C (BatchedHumanoidEnv.reset_footsteps) in place of the one plain reset.  The
 graph body is unchanged: the accumulator's footsteps-reached and sequence-length words already give each cell's progress.
+
+The latency sweep (`eval --num-envs N --action-delays 0,0.005,0.01,0.02,0.025`, DESIGN.md §7.9) gives env i the action delay of
+cell i mod C (BatchedHumanoidEnv.set_action_delay) after the reset, before the first step and outside the graph.  Autoreset is off,
+so nothing redraws it; the graph body is unchanged but for its step, which is the delayed one.  Each cell's statistics are
+summarize()'s over its envs.
 """
 from __future__ import annotations
 
@@ -71,15 +76,21 @@ def footstep_grid(n: int, cells):
             np.asarray([v for _, v in cells], dtype=np.float64)[c])
 
 
+def delay_grid(n: int, delays) -> np.ndarray:
+    """Per env the action delay in seconds of the latency sweep: env i is in cell i mod C of delays."""
+    return np.asarray(delays, dtype=np.float64)[np.arange(n) % len(delays)]
+
+
 @torch.no_grad()
-def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None):
+def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None, delay=None):
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
     [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
     push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
     change d [N, 2] (BatchedHumanoidEnv.push); with push=None nothing but the control steps is launched.
     command = (mode [N], ref [N, 3]): held commands (BatchedHumanoidEnv.set_command) applied after the reset, and every step also
     adds to the [N, C_WORDS] signed-velocity records; then the return is (accumulators, signed-velocity records).
-    footsteps = (mode [N], value [N]): the reset is BatchedHumanoidEnv.reset_footsteps with these plans instead of reset()."""
+    footsteps = (mode [N], value [N]): the reset is BatchedHumanoidEnv.reset_footsteps with these plans instead of reset().
+    delay = seconds [N]: action delays (BatchedHumanoidEnv.set_action_delay) set after the reset."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
     if command is not None and env.command_words() != C_WORDS:
@@ -92,6 +103,8 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None
         env.reset()
     if command is not None:
         env.set_command(*command)
+    if delay is not None:
+        env.set_action_delay(delay)
     state = env.obs.float().clone()
     push_k, push_d = push if push is not None else (None, None)
     if push is not None:
@@ -273,6 +286,41 @@ def format_footstep_table(f: dict) -> str:
     return "\n".join(lines)
 
 
+def delay_summary(acc: np.ndarray, delay: np.ndarray, delays, env_name: str, reward_names) -> dict:
+    """The latency sweep's outcome per cell: the delay in seconds, n, and summarize()'s fall fraction, episode length, return,
+    per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the cell's envs."""
+    out = []
+    for d in delays:
+        s = summarize(acc[delay == float(d)], env_name, reward_names)
+        cell = dict(delay=float(d), n=s["num_envs"], fall_fraction=s["fall_fraction"], mean_length=s["length"]["mean"],
+                    return_mean=s["return"]["mean"])
+        cell.update({k: s[k] for k in ("tracking", "footsteps") if k in s})
+        out.append(cell)
+    return dict(delays=[float(d) for d in delays], cells=out)
+
+
+def format_delay_table(d: dict) -> str:
+    f = lambda v: "      -" if v is None else f"{v:7.4f}"
+    lines = ["  action delays: per cell the fall fraction, mean episode length and return"
+             + ("; |v_fwd - vx_ref| per tracked mode" if "tracking" in d["cells"][0] else "")
+             + ("; footsteps reached and sequences completed" if "footsteps" in d["cells"][0] else "")]
+    head = "    delay ms      n   fell  length    return"
+    if "tracking" in d["cells"][0]:
+        head += "".join(f"  {m:>9s}" for m in d["cells"][0]["tracking"])
+    if "footsteps" in d["cells"][0]:
+        head += "     reached  completed"
+    lines.append(head)
+    for x in d["cells"]:
+        row = f"    {1000 * x['delay']:8.1f} {x['n']:>6d} {x['fall_fraction']:6.3f} {x['mean_length']:7.1f} {x['return_mean']:9.3f}"
+        if "tracking" in x:
+            row += "".join(f"    {f(t['vx_error'])}" for t in x["tracking"].values())
+        if "footsteps" in x:
+            fs = x["footsteps"]
+            row += f"  {fs['mean_reached']:5.2f}/{fs['mean_sequence_length']:<5.2f} {fs['completed_fraction']:8.3f}"
+        lines.append(row)
+    return "\n".join(lines)
+
+
 def format_table(s: dict, max_traj_len: int) -> str:
     L = s["length"]
     lines = [f"{s['num_envs']} environments, one episode each, horizon {max_traj_len} control steps",
@@ -294,16 +342,17 @@ def format_table(s: dict, max_traj_len: int) -> str:
 
 
 def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None,
-                     footsteps=None) -> dict:
+                     footsteps=None, delays=None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
     out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
     push-recovery sweep, with its table and `summary.push`.  commands = [(mode name, value), ...]: the command-tracking sweep
     (env i holds the command of cell i mod len(commands)), with its table and `summary.commands`.  footsteps = [(plan type name,
     value), ...]: the footstep sweep (env i resets with the plan of cell i mod len(footsteps)), with its table and
-    `summary.footsteps_sweep`.  Returns the report."""
-    if sum(x is not None for x in (push, commands, footsteps)) > 1:
-        raise ValueError("the push sweep, the command sweep and the footstep sweep are separate evaluations")
-    sweep = held = plans = None
+    `summary.footsteps_sweep`.  delays = [seconds, ...]: the latency sweep (env i has the action delay of cell i mod len(delays)),
+    with its table and `summary.delay`.  Returns the report."""
+    if sum(x is not None for x in (push, commands, footsteps, delays)) > 1:
+        raise ValueError("the push, command, footstep and latency sweeps are separate evaluations")
+    sweep = held = plans = delay = None
     if push is not None:
         k = int(round(push["push_at"] / env.dt))
         speed, dir_deg = push_grid(env.num_envs, push["speeds"], push["directions"])
@@ -314,7 +363,9 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
     if footsteps is not None:
         fs_mode, fs_value = footstep_grid(env.num_envs, footsteps)
         plans = (fs_mode, fs_value)
-    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans)
+    if delays is not None:
+        delay = delay_grid(env.num_envs, delays)
+    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans, delay=delay)
     acc, cacc = (out[0].cpu().numpy(), out[1].cpu().numpy()) if commands is not None else (out.cpu().numpy(), None)
     summary = summarize(acc, env.model_name, env.reward_names)
     pe = per_env(acc, env.model_name, env.reward_names)
@@ -333,6 +384,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         summary["footsteps_sweep"] = footstep_summary(acc, fs_mode, fs_value, footsteps)
         pe.update(footstep_mode=[FOOTSTEP_MODES[m] for m in fs_mode], footstep_value=fs_value.tolist())
         print(format_footstep_table(summary["footsteps_sweep"]))
+    if delays is not None:
+        summary["delay"] = delay_summary(acc, delay, delays, env.model_name, env.reward_names)
+        pe.update(action_delay=delay.tolist())
+        print(format_delay_table(summary["delay"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
                   max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:

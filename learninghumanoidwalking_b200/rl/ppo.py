@@ -30,6 +30,10 @@ from .snapshot import SnapshotError, plain_args
 from .storage import BatchData
 from .workers import DeviceRolloutWorker
 
+# per-env int32 tensors an env may own beside its records (None when off), which a snapshot shard then holds too: the name, what
+# it is and the training flag that turns it on
+_PER_ENV = {"stair_level": ("stair levels", "--stair-curriculum"), "action_delay": ("action delays", "--action-delay")}
+
 
 class _FusedPPOLoss(torch.autograd.Function):
     """The loss tail of update_actor_critic (rl/algos/ppo.py:302-386) as ONE launch (csrc/ppo_kernels.cu: ppo_loss_kernel): the 7
@@ -204,7 +208,7 @@ class PPO:
                     num_envs=env.num_envs, model=env.model_name, precision=env.precision, seed=env.seed,
                     state_r=env.state_r.cpu(), state_i=env.state_i.cpu(), fresh=bool(env._fresh),
                     worker=self.workers[0].state_dict(), cpu_rng=torch.get_rng_state(),
-                    **({} if getattr(env, "stair_level", None) is None else dict(stair_level=env.stair_level.cpu())))
+                    **{name: getattr(env, name).cpu() for name in _PER_ENV if getattr(env, name, None) is not None})
 
     def restore(self, run_dir) -> int:
         """Load the last complete snapshot of `run_dir` into this freshly built PPO and its environment and return the iteration
@@ -227,13 +231,13 @@ class PPO:
             if have.shape != want.shape or have.dtype != want.dtype:
                 raise SnapshotError(f"{name} of the snapshot is {tuple(have.shape)} {have.dtype}, this run has "
                                     f"{tuple(want.shape)} {want.dtype}")
-        stair_level = getattr(env, "stair_level", None)
-        if stair_level is not None:
-            if "stair_level" not in shard:
-                raise SnapshotError("the snapshot holds no stair levels (was it written by a run without --stair-curriculum?)")
-            if shard["stair_level"].shape != stair_level.shape or shard["stair_level"].dtype != stair_level.dtype:
-                raise SnapshotError(f"stair_level of the snapshot is {tuple(shard['stair_level'].shape)} {shard['stair_level'].dtype}, "
-                                    f"this run has {tuple(stair_level.shape)} {stair_level.dtype}")
+        per_env = {name: getattr(env, name) for name in _PER_ENV if getattr(env, name, None) is not None}
+        for name, mine in per_env.items():
+            if name not in shard:
+                raise SnapshotError(f"the snapshot holds no {_PER_ENV[name][0]} (was it written by a run without {_PER_ENV[name][1]}?)")
+            if shard[name].shape != mine.shape or shard[name].dtype != mine.dtype:
+                raise SnapshotError(f"{name} of the snapshot is {tuple(shard[name].shape)} {shard[name].dtype}, "
+                                    f"this run has {tuple(mine.shape)} {mine.dtype}")
         with torch.no_grad():
             self._flat_param.copy_(learner["flat_param"])
             self._flat_m.copy_(learner["exp_avg"])
@@ -243,8 +247,8 @@ class PPO:
                 getattr(getattr(self, net), name).copy_(v)
             env.state_r.copy_(shard["state_r"])
             env.state_i.copy_(shard["state_i"])
-            if stair_level is not None:
-                stair_level.copy_(shard["stair_level"])
+            for name, mine in per_env.items():
+                mine.copy_(shard[name])
         env._fresh = bool(shard["fresh"])
         a_opt.step_count, c_opt.step_count = learner["step_count"]
         if getattr(self, "schedule", "fixed") == "adaptive":

@@ -78,6 +78,8 @@ TRAIN_FLAGS = [
     ("--push-interval", dict(type=_F, default=15.0, help="mean seconds between two random pushes of an env")),
     ("--stair-curriculum", dict(type=_F, default=0.0, help="jvrc_step: a stair level per env up to H m, a multiple of 0.01 in (0, 0.2], "
                                                            "moved by each FORWARD episode (0: off, the reference's schedule; DESIGN §7.8)")),
+    ("--action-delay", dict(type=_F, default=0.0, help="random action delays: every reset draws its env's delay uniformly from whole "
+                                                       "physics substeps in [0, S] s, S <= control_dt (0: off; DESIGN §7.9)")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -101,7 +103,11 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
               ("--footsteps", dict(type=_S, nargs="+", action="extend", default=None,
                                    help="jvrc_step footstep plans TYPE[:v1,v2,...]: forward:H (signed stair height, m), "
                                         "lateral:left,right, curved[:plan index,...], backward, standing; with --num-envs one cell "
-                                        "per (type, value), else exactly one"))]
+                                        "per (type, value), else exactly one")),
+              # the latency sweep (DESIGN §7.9)
+              ("--action-delays", dict(type=_S, default=None,
+                                       help="comma-separated action delays in s, whole physics substeps up to control_dt, e.g. "
+                                            "0,0.005,0.01,0.02,0.025; with --num-envs one cell per delay, else exactly one"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -128,6 +134,8 @@ def print_system_info(args, training=True):
         stairs = getattr(args, "stair_curriculum", 0.0)
         if stairs:
             print(f"Stair curriculum: levels of 0.01 m up to {stairs} m")
+        delay = getattr(args, "action_delay", 0.0)
+        print(f"Action delays: up to {delay * 1000:g} ms, drawn at every reset" if delay > 0 else "Action delays: off")
     print("=" * 60)
 
 
@@ -176,7 +184,8 @@ def make_env_fn(args, rank, world, local):
     env_fn = partial(Env, n_local, precision=args.precision, seed=seed, first_env_id=first, device=local,
                      max_traj_len=args.max_traj_len, path_to_yaml=args.yaml, push_vel=getattr(args, "push_vel", 0.0),
                      push_interval=getattr(args, "push_interval", 15.0),   # an experiment.pkl without them: no pushes
-                     stair_curriculum=getattr(args, "stair_curriculum", 0.0))   # nor a stair curriculum
+                     stair_curriculum=getattr(args, "stair_curriculum", 0.0),   # nor a stair curriculum
+                     action_delay=getattr(args, "action_delay", 0.0))   # nor action delays
     _env = env_fn()
     if not args.no_mirror:
         try:
@@ -231,10 +240,34 @@ def check_stairs(args):
         raise SystemExit(f"train --stair-curriculum {stairs}: {e}")
 
 
+def check_action_delay(args):
+    """Refuse a largest action delay the env would refuse (checked against the model after --yaml), before any environment or
+    run directory exists."""
+    from learninghumanoidwalking_b200.envs.batched_env import action_delay_substeps
+    delay = getattr(args, "action_delay", 0.0)
+    cfg = _run_cfg(args.env, args.yaml)
+    try:
+        action_delay_substeps(delay, cfg["sim_dt"], cfg["control_dt"])
+    except ValueError as e:
+        raise SystemExit(f"train --action-delay {delay}: {e}")
+
+
+def _run_cfg(env_name, yaml):
+    """The model's cfg block after the user's YAML, as the env applies it."""
+    from learninghumanoidwalking_b200.model import load_model
+    import_env(env_name)
+    mj = load_model(env_name)
+    if yaml is not None:
+        from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
+        mj = apply_config(mj, load_yaml(yaml))
+    return mj["cfg"]
+
+
 def run_experiment(args):
     from learninghumanoidwalking_b200.rl import PPO
     check_push(args)
     check_stairs(args)
+    check_action_delay(args)
     rank, world, local = _dist_setup()
     timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
     args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
@@ -455,6 +488,39 @@ def footstep_cells(args):
     return cells
 
 
+def delay_cells(args):
+    """The action delays of `eval --action-delays ...` in seconds, or None without the flag; the grammar and the combinations are
+    refused here, the values against the run's model by check_delays."""
+    if args.action_delays is None:
+        return None
+    try:
+        cells = [float(v) for v in args.action_delays.split(",")]
+    except ValueError:
+        raise SystemExit(f"eval --action-delays {args.action_delays!r}: expected comma-separated delays in s, e.g. 0,0.005,0.01,0.02")
+    if not all(v >= 0 and v < float("inf") for v in cells):
+        raise SystemExit(f"eval --action-delays {args.action_delays}: every delay must be finite and >= 0")
+    if args.push_speeds is not None or args.command is not None or args.footsteps is not None:
+        raise SystemExit("eval --action-delays, --push-speeds, --command and --footsteps are separate sweeps: run them one at a time")
+    if args.num_envs is None and len(cells) != 1:
+        raise SystemExit(f"eval --action-delays: {len(cells)} delays need the batched evaluation (add --num-envs N); the single-env "
+                         "roll-out takes exactly one")
+    if args.num_envs is not None and args.num_envs < len(cells):
+        raise SystemExit(f"eval --num-envs {args.num_envs}: --action-delays lists {len(cells)} cells, and every cell needs at least "
+                         "one environment")
+    return cells
+
+
+def check_delays(delays, run_args, yaml):
+    """Refuse delays the run's env would refuse (whole substeps of its sim_dt, at most its control_dt), before the actor is
+    loaded."""
+    from learninghumanoidwalking_b200.envs.batched_env import action_delay_substeps
+    cfg = _run_cfg(run_args.env, yaml)
+    try:
+        action_delay_substeps(delays, cfg["sim_dt"], cfg["control_dt"])
+    except ValueError as e:
+        raise SystemExit(f"eval --action-delays: {e}")
+
+
 def check_footstep_env(env_name):
     """Refuse --footsteps for a run whose env is not jvrc_step, before its actor is loaded."""
     if env_name != "jvrc_step":
@@ -471,6 +537,7 @@ def evaluate_batched(args):
     push = push_sweep(args)
     commands = command_cells(args)
     footsteps = footstep_cells(args)
+    delays = delay_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -482,6 +549,8 @@ def evaluate_batched(args):
     yaml = run_args.yaml
     if yaml is not None and Path(path_to_actor.parent, Path(yaml).name).exists():
         yaml = str(Path(path_to_actor.parent, Path(yaml).name))      # the copy that rode along with the run, as `resume` uses
+    if delays is not None:
+        check_delays(delays, run_args, yaml)
     if push is not None:       # the push step needs the run's control step and horizon; refused before the actor is loaded
         from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
         from learninghumanoidwalking_b200.model import load_model
@@ -501,7 +570,7 @@ def evaluate_batched(args):
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
     report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands,
-                 footsteps=footsteps)
+                 footsteps=footsteps, delays=delays)
     env.close()
     return report
 
@@ -516,6 +585,7 @@ def evaluate(args):
         raise SystemExit("eval --push-speeds, --push-directions and --push-at belong to the batched evaluation: add --num-envs N")
     commands = command_cells(args)
     footsteps = footstep_cells(args)
+    delays = delay_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -524,6 +594,8 @@ def evaluate(args):
         check_command_env(run_args.env)
     if footsteps is not None:
         check_footstep_env(run_args.env)
+    if delays is not None:
+        check_delays(delays, run_args, None)     # the single-env roll-out runs the env's own model, as it always has
     cv2 = None
     if args.out_dir is not None:
         try:
@@ -547,6 +619,8 @@ def evaluate(args):
             from learninghumanoidwalking_b200.rl.evaluation import command_grid, command_refs
             mode, value = command_grid(1, commands)
             env.set_command(mode, command_refs(mode, value))
+        if delays is not None:       # the one delay, set again after every reset
+            env.set_action_delay(delays)
         return env.obs.float()
 
     obs = reset()
