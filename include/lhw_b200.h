@@ -175,6 +175,27 @@ int lhw_sim_step_delay(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs
 int lhw_sim_draw_delay(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
                        int max_delay, int32_t* delay, void* stream);
 
+/* lhw_sim_step_payload: lhw_sim_step with a payload carried by each env's root link (DESIGN.md §7.10), every variant.  payload
+ * [n][4] (device, the sim's precision) holds each env's (m, rx, ry, rz): a point mass m >= 0 kg rigidly attached to the root link
+ * at r (m), given in the root link's frame relative to the compiled model's root-link centre of mass.  It is read once per control
+ * step.  Every physics substep of the control step builds the root link's mass, centre of mass and inertia as the composite of
+ * the link and the point mass (H1: on top of the env's randomised link); an auto-reset's settling substeps run without it.
+ * Observations, rewards, termination and the contact regularisation constants are unchanged.  An env whose mass is exactly 0 is
+ * lhw_sim_step bit for bit, whatever its offset.  delay [n] (device int32, or NULL for none) adds the action delays of
+ * lhw_sim_step_delay; level != NULL (jvrc_step only) adds the stair curriculum of lhw_sim_step_stairs, with its refusals.
+ * Nothing writes payload or delay.
+ * lhw_sim_draw_payload: the random payloads.  Every env whose mask [n] word is non-zero (every env when mask is NULL; pass the
+ * step's `ended`, or a reset's mask) gets payload[i] = (max_mass u01(u[0]), max_offset (2 u01(u[1..3]) - 1)) with
+ * u = philox(seed, first_env_id + i, rng_ctr, 72), rng_ctr the record's event counter (state_i[i][4]) as the reset left it.
+ * Only payload is written.  max_mass not finite or negative, or max_offset outside [0, 0.25], is refused with -2; the host
+ * bounds max_mass by half the robot's mass.  Reads no model constants. */
+int lhw_sim_step_payload(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                         const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
+                         void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, const void* payload,
+                         const int32_t* delay, int32_t* level, int n_levels, void* stream);
+int lhw_sim_draw_payload(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
+                         double max_mass, double max_offset, void* payload, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

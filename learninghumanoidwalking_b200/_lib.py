@@ -49,6 +49,11 @@ SIGNATURES = {
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_int, c_void_p]),
     "lhw_sim_draw_delay": (c_int, [c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, c_int, c_void_p, c_void_p]),
+    "lhw_sim_step_payload": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, c_int, c_int,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_int, c_void_p]),
+    "lhw_sim_draw_payload": (c_int, [c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, ctypes.c_double, ctypes.c_double, c_void_p,
+                                     c_void_p]),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

@@ -844,10 +844,53 @@ template <class real, int NJ, int TK> LHW_DEVNI void newton_hessian_f64(Work<rea
   }
 }
 
-// ================================================================= one physics substep (mujoco.mj_step)
+// ================================================================= carried payload (lhw_sim_step_payload, DESIGN.md §7.10)
+// A point mass m >= 0 kg rigidly attached to the root link at r, given in the root link's frame relative to the compiled model's
+// root-link centre of mass com[0].  The payload step kernels read an env's four words (m, rx, ry, rz) once per control step and
+// hand them to every substep.
+template <class real> struct Payload { real m, r[3]; };
+
+// the plain link-inertia build: no payload
 template <class real, int NJ, int TK>
+LHW_DEV void root_payload(const Work<real, NJ, TK>&, const Model<real, NJ, TK>&, int, const real*, real&, real*, real*) {}
+
+// Link i's mass ms, its centre of mass c (rotated to world axes by R, before the link origin is added) and its inertia Ib about
+// that centre (link frame) become the composite of the root link and the payload pl.  Only the root link (i == 0) carries one,
+// and a payload of mass exactly 0 leaves the plain build's values alone, whatever its offset.  With p = com[0] + r and the root
+// link's (ms, c, Ib) as the build has them (H1: the env's randomised p_mass[0], p_com[0], p_inertia0):
+//   M' = ms + m,  c' = (ms c + m p) / M',  I' = Ib + ms (|c - c'|^2 E - (c - c')(c - c')^T) + m (|p - c'|^2 E - (p - c')(p - c')^T)
+template <class real, int NJ, int TK>
+LHW_DEV void root_payload(const Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, int i, const real* R, real& ms, real* c,
+                          real* Ib, const Payload<real>& pl) {
+  if (i != 0 || pl.m == 0) return;
+  real cl[3], cc[3], d1[3], d2[3];
+#pragma unroll
+  for (int x = 0; x < 3; x++) {
+    const real c0 = LHW_GLD(m, com[0][x]);
+    if constexpr (Cfg<NJ, TK>::PERENV) cl[x] = w.p_com[0][x];
+    else cl[x] = c0;
+    const real p = c0 + pl.r[x];
+    cc[x] = (ms * cl[x] + pl.m * p) / (ms + pl.m);
+    d1[x] = cl[x] - cc[x];
+    d2[x] = p - cc[x];
+  }
+  const real a1 = dot3(d1, d1), a2 = dot3(d2, d2);
+  Ib[0] += ms * (a1 - d1[0] * d1[0]) + pl.m * (a2 - d2[0] * d2[0]);
+  Ib[1] += ms * (a1 - d1[1] * d1[1]) + pl.m * (a2 - d2[1] * d2[1]);
+  Ib[2] += ms * (a1 - d1[2] * d1[2]) + pl.m * (a2 - d2[2] * d2[2]);
+  Ib[3] -= ms * d1[0] * d1[1] + pl.m * d2[0] * d2[1];
+  Ib[4] -= ms * d1[0] * d1[2] + pl.m * d2[0] * d2[2];
+  Ib[5] -= ms * d1[1] * d1[2] + pl.m * d2[1] * d2[2];
+  ms += pl.m;
+  mv3(R, cc, c);
+}
+
+// ================================================================= one physics substep (mujoco.mj_step)
+// PL: empty (the plain step) or one Payload<real> (the root link carries it; root_payload above).  The pack keeps the plain
+// instantiations' parameter list, and so their code, as it was.
+template <class real, int NJ, int TK, class... PL>
 LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, const bool last, const int block_sync = 0,
-                       const bool chained = false) {
+                       const bool chained = false, const PL... pl) {
   constexpr int NL = 1 + 2 * NJ, NV = 6 + 2 * NJ, NU = 2 * NJ, NA = 6 + NJ;
   constexpr int CPF = Cfg<NJ, TK>::CPF, NCON = 2 * CPF, NEDGE = 4 * NCON, NPTS = Cfg<NJ, TK>::NPTS;
   constexpr bool PERENV = Cfg<NJ, TK>::PERENV, FLOSS = Cfg<NJ, TK>::FLOSS;
@@ -954,6 +997,7 @@ LHW_DEVNI void substep(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m_arg, 
         mv3(R, cm, c);
         ms = LHW_GLD(m, mass[i]);
       }
+      root_payload(w, m, i, R, ms, c, Ib, pl...);
 #pragma unroll
       for (int x = 0; x < 3; x++) c[x] += w.xr[i][x];
       const real B[9] = {Ib[0], Ib[3], Ib[4], Ib[3], Ib[1], Ib[5], Ib[4], Ib[5], Ib[2]};
@@ -2246,12 +2290,14 @@ LHW_DEV int action_delay_clamp(int d, int frame_skip) { return d < 0 ? 0 : d > f
 // only, DESIGN.md §7.8): *level is the env's stair-curriculum level of n_levels; an auto-reset first moves it by the ending episode
 // when that was a FORWARD one (stair_level_next), then resets with its stair height.  DELAY (DESIGN.md §7.9): substeps
 // 0 .. delay-1 drive the PD loop towards the previous control step's target (prev_action, which holds it until the record update
-// below), the rest towards this step's; delay is already clamped to [0, frame_skip].  At delay 0 the step is the plain one
-template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false>
+// below), the rest towards this step's; delay is already clamped to [0, frame_skip].  At delay 0 the step is the plain one.
+// PAYLOAD (DESIGN.md §7.10): every substep of the step builds the root link with the payload pay (root_payload); an auto-reset's
+// settling substeps do not.  A payload of mass 0 is the plain step
+template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false>
 LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const real* action, uint32_t seed, int max_traj_len,
                       int autoreset, const int block_sync, const int alive, real* obs_out, real* term_obs_out, real* reward_out, real* rew_terms_out,
                       int32_t* done_out, int32_t* ended_out, int32_t* ep_len_out, real* ep_rew_out, int32_t* level = nullptr,
-                      int n_levels = 0, const int delay = 0) {
+                      int n_levels = 0, const int delay = 0, const Payload<real> pay = {}) {
   constexpr int NU = 2 * NJ, NOBS = Work<real, NJ, TK>::NOBS;
   // action smoothing + nominal offsets (base_humanoid_env.py:209-212, robot_base.py:80-85)
   // one event counter per control step: every draw of this step is keyed by rng_ctr + 1 (stored below)
@@ -2287,8 +2333,13 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
       }
     }
     LHW_SYNC();
-    if (alive) substep<real, NJ, TK>(w, m, sidx == m.frame_skip - 1, block_sync, sidx > 0);
-    else LHW_BLOCK_SYNC(block_sync & 2);
+    if constexpr (PAYLOAD) {
+      if (alive) substep<real, NJ, TK>(w, m, sidx == m.frame_skip - 1, block_sync, sidx > 0, pay);
+      else LHW_BLOCK_SYNC(block_sync & 2);
+    } else {
+      if (alive) substep<real, NJ, TK>(w, m, sidx == m.frame_skip - 1, block_sync, sidx > 0);
+      else LHW_BLOCK_SYNC(block_sync & 2);
+    }
     LHW_BLOCK_SYNC((block_sync & 1) && ((sidx + 1) % ((block_sync >> 4) + 1) == 0));   // every (block_sync>>4)+1 substeps
   }
   if (!alive) return;
@@ -2609,7 +2660,8 @@ LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward,
 // joint velocities are unchanged.  Nothing else of the record is written, and nothing of an env that is not pushed.
 // The random pushes draw on their own Philox stream at the env's event counter, which they only read.  The step and reset
 // bodies above draw on streams 0-5, 8-13, 16-35, 40-48, 50-54 and 60-64, so with pushes off every trajectory is unchanged.
-// The random action delays draw on stream 71 (DELAY_STREAM, delay_draw_env below).
+// The random action delays draw on stream 71 (DELAY_STREAM, delay_draw_env below), the random payloads on stream 72
+// (PAYLOAD_STREAM, payload_draw_env below).
 constexpr uint32_t PUSH_STREAM = 70;
 
 // One env's push; returns 1 when it was pushed.  Explicit mode (d != nullptr): (dx, dy) = (d[0], d[1]), skipped when both are
@@ -2656,6 +2708,25 @@ LHW_DEV void delay_draw_env(const int32_t* si, uint32_t seed, uint32_t env_id, i
   uint32_t u[4];
   philox(seed, env_id, (uint32_t)si[4], DELAY_STREAM, u);
   *delay = randint(u[0], max_delay + 1);
+}
+
+// ================================================================= random payloads (lhw_sim_draw_payload, DESIGN.md §7.10)
+// An env that was just reset (sel != 0: its ended word or mask word) draws the payload of its new episode: with
+// u = philox(seed, env_id, rng_ctr, PAYLOAD_STREAM) at the event counter the reset left (si[4]), mass m = max_mass u01(u[0]) and
+// offset r_k = max_offset (2 u01(u[1 + k]) - 1), so m ~ U(0, max_mass) and r ~ U(-max_offset, max_offset)^3.  The arithmetic is
+// float64 at either precision, rounded once to the payload's precision.  Only pay[0..3] = (m, rx, ry, rz) is written.
+constexpr uint32_t PAYLOAD_STREAM = 72;
+constexpr double PAYLOAD_MAX_OFFSET = 0.25;   // m: the largest offset component of a payload
+
+template <class real>
+LHW_DEV void payload_draw_env(const int32_t* si, uint32_t seed, uint32_t env_id, int32_t sel, double max_mass, double max_offset,
+                              real* pay) {
+  if (!sel) return;
+  uint32_t u[4];
+  philox(seed, env_id, (uint32_t)si[4], PAYLOAD_STREAM, u);
+  pay[0] = (real)(max_mass * u01<double>(u[0]));
+#pragma unroll
+  for (int k = 0; k < 3; k++) pay[1 + k] = (real)(max_offset * (2 * u01<double>(u[1 + k]) - 1));
 }
 
 // ================================================================= held commands (lhw_sim_set_command, DESIGN.md §7.6)

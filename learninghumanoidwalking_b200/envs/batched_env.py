@@ -87,6 +87,36 @@ def action_delay_substeps(seconds, sim_dt: float, control_dt: float) -> np.ndarr
     return k.astype(np.int32)
 
 
+PAYLOAD_MAX_OFFSET = 0.25   # m: the largest payload offset component (csrc/sim_core.h PAYLOAD_MAX_OFFSET)
+
+
+def check_payload(mass, offset, total_mass: float) -> tuple[np.ndarray, np.ndarray]:
+    """Payload masses (kg, a number or a sequence) and offsets (m, a number or a sequence of numbers or of triples) as float64
+    arrays, after refusing a mass that is negative, not finite or above half the robot's total_mass, and an offset component that
+    is not finite or whose magnitude is above PAYLOAD_MAX_OFFSET (DESIGN.md §7.10)."""
+    m = np.asarray(mass, dtype=np.float64).reshape(-1)
+    r = np.asarray(offset, dtype=np.float64)
+    bad = ~np.isfinite(m) | (m < 0) | (m > 0.5 * total_mass)
+    if bad.any():
+        raise ValueError(f"a payload mass must lie in [0, {0.5 * total_mass:g}] kg (half the robot's {total_mass:g} kg), "
+                         f"got {m[bad][0]}")
+    bad = ~np.isfinite(r) | (np.abs(r) > PAYLOAD_MAX_OFFSET)
+    if bad.any():
+        raise ValueError(f"a payload offset must lie in [-{PAYLOAD_MAX_OFFSET:g}, {PAYLOAD_MAX_OFFSET:g}] m per axis, "
+                         f"got {r[bad].reshape(-1)[0]}")
+    return m, r
+
+
+def check_payload_range(mass: float, offset: float, total_mass: float) -> None:
+    """Refuse the random payloads' ranges M (mass U(0, M)) and R (offset U(-R, R)^3) that check_payload refuses as values, a
+    negative R, and an R without an M."""
+    check_payload(mass, offset, total_mass)
+    if offset < 0:
+        raise ValueError(f"a payload offset range must be >= 0 m, got {offset}")
+    if offset and not mass:
+        raise ValueError("a payload offset range needs a payload mass range")
+
+
 class _Robot(SimpleNamespace):
     """The attributes the trainer reads / writes on `env.robot` (robots/robot_base.py:35, run_experiment.py:123-125).
     Writing `iteration_count` (rl/workers/rollout_worker.py:95) drives the SteppingTask's height curriculum."""
@@ -103,7 +133,8 @@ class BatchedHumanoidEnv:
                  tolerance: float | None = None, max_iter: int | None = None, observation_noise: bool = True,
                  domain_randomization: bool = True, init_noise: bool = True, pd_gain_randomization: float = 0.0,
                  iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0,
-                 stair_curriculum: float = 0.0, action_delay: float = 0.0):
+                 stair_curriculum: float = 0.0, action_delay: float = 0.0, payload_mass: float = 0.0,
+                 payload_offset: float = 0.0):
         # a stair level per env (DESIGN.md §7.8): every reset builds a FORWARD plan with its level's stair height, and each
         # auto-reset first moves the level by the ending FORWARD episode; off at 0, and then the launches are the plain ones
         self.stair_levels = stair_levels(model, stair_curriculum)
@@ -128,6 +159,10 @@ class BatchedHumanoidEnv:
         self.push_interval_steps = push_interval_steps(push_vel, push_interval, self.mj["cfg"]["control_dt"])
         # random action delays (DESIGN.md §7.9): every reset draws its env's delay from U{0 .. action_delay_max} substeps
         self.action_delay_max = int(action_delay_substeps(action_delay, self.mj["cfg"]["sim_dt"], self.mj["cfg"]["control_dt"])[0])
+        # random payloads (DESIGN.md §7.10): every reset draws its env's payload, mass U(0, payload_mass), offset
+        # U(-payload_offset, payload_offset)^3 on the root link
+        check_payload_range(payload_mass, payload_offset, self.mj["total_mass"])
+        self.payload_mass, self.payload_offset = float(payload_mass), float(payload_offset)
         if tolerance is None and precision == 32:
             tolerance = 1e-6  # fp32 cannot reach the reference's 1e-10; gradient floor is ~1e-6 of the force scale
         flat = pack_model(self.mj, tolerance=tolerance, max_iter=max_iter, observation_noise=observation_noise,
@@ -156,6 +191,9 @@ class BatchedHumanoidEnv:
         # int32 [N]: each env's action delay in physics substeps; None (and the plain step kernels) until random delays or
         # set_action_delay create it
         self.action_delay = torch.zeros(n, dtype=torch.int32, device=dev) if self.action_delay_max else None
+        # [N, 4] of the env's dtype: each env's payload (m, rx, ry, rz); None (and the plain step kernels) until random payloads or
+        # set_payload create it
+        self.payload = torch.zeros(n, 4, dtype=self.dtype, device=dev) if self.payload_mass else None
         # ---- reference-facing attributes (envs/jvrc/jvrc_base.py:69-131, envs/jvrc/jvrc_walk.py:43-63)
         cfg = self.mj["cfg"]
         self.history_len = cfg["obs_history_len"]
@@ -237,6 +275,7 @@ class BatchedHumanoidEnv:
         if mask is None:
             self._fresh = False
         self._draw_delay(0, self.num_envs, mask)
+        self._draw_payload(0, self.num_envs, mask)
         return self.obs
 
     def step(self, actions: torch.Tensor, autoreset: bool = True):
@@ -244,6 +283,9 @@ class BatchedHumanoidEnv:
         With autoreset the RolloutWorker semantics apply (see include/lhw_b200.h: lhw_sim_step)."""
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
+        if self.payload is not None:
+            self._step_payload(0, self.num_envs, actions, autoreset)
+            return self.obs, self.reward, self.done, self.ended
         if self.action_delay is not None:
             self._step_delay(0, self.num_envs, actions, autoreset)
             return self.obs, self.reward, self.done, self.ended
@@ -279,6 +321,9 @@ class BatchedHumanoidEnv:
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
         out = (self.obs[sl], self.reward[sl], self.done[sl], self.ended[sl])
+        if self.payload is not None:
+            self._step_payload(lo, hi, actions, autoreset)
+            return out
         if self.action_delay is not None:
             self._step_delay(lo, hi, actions, autoreset)
             return out
@@ -337,6 +382,47 @@ class BatchedHumanoidEnv:
         if self.action_delay is None:
             self.action_delay = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         self.action_delay.copy_(torch.from_numpy(d))
+
+    def _step_payload(self, lo: int, hi: int, actions: torch.Tensor, autoreset: bool) -> None:
+        """The control step of environments [lo, hi) with their payloads (and their action delays and stair levels when those
+        are on), then, with autoreset, the random draws of the envs it ended (and so reset), then the random pushes; all on the
+        current stream."""
+        sl = slice(lo, hi)
+        delay = None if self.action_delay is None else self.action_delay[sl]
+        level = None if self.stair_level is None else self.stair_level[sl]
+        _lib.ops().sim_step_payload(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
+                                    self.max_traj_len, bool(autoreset), self.obs[sl], self.term_obs[sl], self.reward[sl],
+                                    self.rew_terms[sl], self.done[sl], self.ended[sl], self.ep_len[sl], self.ep_rew[sl],
+                                    self.payload[sl], delay, level, self.stair_levels)
+        if autoreset:
+            self._draw_delay(lo, hi, self.ended[sl])
+            self._draw_payload(lo, hi, self.ended[sl])
+        self._push_random(lo, hi)
+
+    def _draw_payload(self, lo: int, hi: int, mask: torch.Tensor | None) -> None:
+        """Random mode: environments [lo, hi) whose mask word is non-zero (all without a mask), just reset, draw their new
+        episode's payload; nothing is launched otherwise (include/lhw_b200.h: lhw_sim_draw_payload)."""
+        if self.payload_mass:
+            _lib.ops().sim_draw_payload(self._h.value, self.state_i[lo:hi], self.seed, self.first_env_id + lo, mask, self.payload_mass,
+                                        self.payload_offset, self.payload[lo:hi])
+
+    def set_payload(self, mass, offset=None) -> None:
+        """Give every environment a payload on its root link: mass holds N values in kg (a sequence or tensor), offset None (at
+        the root link's centre of mass), one (x, y, z) for every env or [N, 3], in m in the root link's frame relative to the
+        compiled model's root-link centre of mass.  A mass is at most half the robot's total_mass, an offset component at most
+        0.25 m in magnitude.  The payloads hold until each env's next reset draws a new one (random mode, payload_mass > 0) or
+        until they are set again (include/lhw_b200.h: lhw_sim_step_payload)."""
+        m = torch.as_tensor(mass, dtype=torch.float64).detach().to("cpu").reshape(-1)
+        if m.shape != (self.num_envs,):
+            raise ValueError(f"mass must hold {self.num_envs} numbers, got {tuple(m.shape)}")
+        r = np.zeros(3) if offset is None else torch.as_tensor(offset, dtype=torch.float64).detach().to("cpu").numpy()
+        if r.shape not in ((3,), (self.num_envs, 3)):
+            raise ValueError(f"offset must be (x, y, z) or [{self.num_envs}, 3], got {tuple(r.shape)}")
+        m, r = check_payload(m.numpy(), r, self.mj["total_mass"])
+        host = np.concatenate([m[:, None], np.broadcast_to(r, (self.num_envs, 3))], axis=1)
+        if self.payload is None:
+            self.payload = torch.zeros(self.num_envs, 4, dtype=self.dtype, device=self.device)
+        self.payload.copy_(torch.from_numpy(host))
 
     def _push_random(self, lo: int, hi: int) -> None:
         """The random pushes of environments [lo, hi) after their control step, on the same stream; none at push_vel == 0.
@@ -414,8 +500,10 @@ class BatchedHumanoidEnv:
                                        mode.to(device=self.device, dtype=torch.int32), value.to(device=self.device, dtype=self.dtype),
                                        self._fresh, self.obs)
         self._fresh = False
-        if self.action_delay_max:
-            self._draw_delay(0, self.num_envs, (mode >= 0).to(device=self.device, dtype=torch.int32))
+        if self.action_delay_max or self.payload_mass:
+            picked = (mode >= 0).to(device=self.device, dtype=torch.int32)
+            self._draw_delay(0, self.num_envs, picked)
+            self._draw_payload(0, self.num_envs, picked)
         return self.obs
 
     def command_accumulate(self, acc: torch.Tensor) -> torch.Tensor:

@@ -23,6 +23,11 @@ The latency sweep (`eval --num-envs N --action-delays 0,0.005,0.01,0.02,0.025`, 
 cell i mod C (BatchedHumanoidEnv.set_action_delay) after the reset, before the first step and outside the graph.  Autoreset is off,
 so nothing redraws it; the graph body is unchanged but for its step, which is the delayed one.  Each cell's statistics are
 summarize()'s over its envs.
+
+The payload sweep (`eval --num-envs N --payloads 0,5,10,15,20 [--payload-at x,y,z]`, DESIGN.md §7.10) gives env i the payload mass
+of cell i mod C, all at the one point --payload-at (BatchedHumanoidEnv.set_payload), after the reset, before the first step and
+outside the graph.  Autoreset is off, so nothing redraws it; the graph body is unchanged but for its step, which is the payload
+one.  Each cell's statistics are summarize()'s over its envs.
 """
 from __future__ import annotations
 
@@ -81,8 +86,13 @@ def delay_grid(n: int, delays) -> np.ndarray:
     return np.asarray(delays, dtype=np.float64)[np.arange(n) % len(delays)]
 
 
+def payload_grid(n: int, masses) -> np.ndarray:
+    """Per env the payload mass in kg of the payload sweep: env i is in cell i mod C of masses."""
+    return np.asarray(masses, dtype=np.float64)[np.arange(n) % len(masses)]
+
+
 @torch.no_grad()
-def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None, delay=None):
+def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None, delay=None, payload=None):
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
     [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
     push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
@@ -90,7 +100,8 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None
     command = (mode [N], ref [N, 3]): held commands (BatchedHumanoidEnv.set_command) applied after the reset, and every step also
     adds to the [N, C_WORDS] signed-velocity records; then the return is (accumulators, signed-velocity records).
     footsteps = (mode [N], value [N]): the reset is BatchedHumanoidEnv.reset_footsteps with these plans instead of reset().
-    delay = seconds [N]: action delays (BatchedHumanoidEnv.set_action_delay) set after the reset."""
+    delay = seconds [N]: action delays (BatchedHumanoidEnv.set_action_delay) set after the reset.
+    payload = (mass [N], offset (x, y, z)): payloads (BatchedHumanoidEnv.set_payload) set after the reset."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
     if command is not None and env.command_words() != C_WORDS:
@@ -105,6 +116,8 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None
         env.set_command(*command)
     if delay is not None:
         env.set_action_delay(delay)
+    if payload is not None:
+        env.set_payload(*payload)
     state = env.obs.float().clone()
     push_k, push_d = push if push is not None else (None, None)
     if push is not None:
@@ -286,32 +299,34 @@ def format_footstep_table(f: dict) -> str:
     return "\n".join(lines)
 
 
-def delay_summary(acc: np.ndarray, delay: np.ndarray, delays, env_name: str, reward_names) -> dict:
-    """The latency sweep's outcome per cell: the delay in seconds, n, and summarize()'s fall fraction, episode length, return,
-    per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the cell's envs."""
+def _cell_summary(acc: np.ndarray, per_env: np.ndarray, values, key: str, env_name: str, reward_names) -> list:
+    """One sweep's outcome per cell: the cell's value under `key`, n, and summarize()'s fall fraction, episode length, return,
+    per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the envs whose per_env value
+    is the cell's."""
     out = []
-    for d in delays:
-        s = summarize(acc[delay == float(d)], env_name, reward_names)
-        cell = dict(delay=float(d), n=s["num_envs"], fall_fraction=s["fall_fraction"], mean_length=s["length"]["mean"],
-                    return_mean=s["return"]["mean"])
+    for v in values:
+        s = summarize(acc[per_env == float(v)], env_name, reward_names)
+        cell = {key: float(v), "n": s["num_envs"], "fall_fraction": s["fall_fraction"], "mean_length": s["length"]["mean"],
+                "return_mean": s["return"]["mean"]}
         cell.update({k: s[k] for k in ("tracking", "footsteps") if k in s})
         out.append(cell)
-    return dict(delays=[float(d) for d in delays], cells=out)
+    return out
 
 
-def format_delay_table(d: dict) -> str:
+def _format_cells(d: dict, title: str, head: str, value) -> str:
+    """The table of a sweep's cells: title, then per cell `value(cell)` followed by _cell_summary's statistics."""
     f = lambda v: "      -" if v is None else f"{v:7.4f}"
-    lines = ["  action delays: per cell the fall fraction, mean episode length and return"
+    lines = [f"  {title}: per cell the fall fraction, mean episode length and return"
              + ("; |v_fwd - vx_ref| per tracked mode" if "tracking" in d["cells"][0] else "")
              + ("; footsteps reached and sequences completed" if "footsteps" in d["cells"][0] else "")]
-    head = "    delay ms      n   fell  length    return"
+    head = f"    {head}      n   fell  length    return"
     if "tracking" in d["cells"][0]:
         head += "".join(f"  {m:>9s}" for m in d["cells"][0]["tracking"])
     if "footsteps" in d["cells"][0]:
         head += "     reached  completed"
     lines.append(head)
     for x in d["cells"]:
-        row = f"    {1000 * x['delay']:8.1f} {x['n']:>6d} {x['fall_fraction']:6.3f} {x['mean_length']:7.1f} {x['return_mean']:9.3f}"
+        row = f"    {value(x)} {x['n']:>6d} {x['fall_fraction']:6.3f} {x['mean_length']:7.1f} {x['return_mean']:9.3f}"
         if "tracking" in x:
             row += "".join(f"    {f(t['vx_error'])}" for t in x["tracking"].values())
         if "footsteps" in x:
@@ -319,6 +334,29 @@ def format_delay_table(d: dict) -> str:
             row += f"  {fs['mean_reached']:5.2f}/{fs['mean_sequence_length']:<5.2f} {fs['completed_fraction']:8.3f}"
         lines.append(row)
     return "\n".join(lines)
+
+
+def delay_summary(acc: np.ndarray, delay: np.ndarray, delays, env_name: str, reward_names) -> dict:
+    """The latency sweep's outcome per cell: the delay in seconds, n, and summarize()'s fall fraction, episode length, return,
+    per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the cell's envs."""
+    return dict(delays=[float(d) for d in delays], cells=_cell_summary(acc, delay, delays, "delay", env_name, reward_names))
+
+
+def format_delay_table(d: dict) -> str:
+    return _format_cells(d, "action delays", "delay ms", lambda x: f"{1000 * x['delay']:8.1f}")
+
+
+def payload_summary(acc: np.ndarray, mass: np.ndarray, masses, at, env_name: str, reward_names) -> dict:
+    """The payload sweep's outcome per cell: the payload mass in kg, n, and summarize()'s fall fraction, episode length, return,
+    per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the cell's envs; `at` is the
+    payload's point, which every cell shares."""
+    return dict(masses=[float(m) for m in masses], at=[float(v) for v in at],
+                cells=_cell_summary(acc, mass, masses, "mass", env_name, reward_names))
+
+
+def format_payload_table(d: dict) -> str:
+    at = ", ".join(f"{v:g}" for v in d["at"])
+    return _format_cells(d, f"payloads at ({at}) m", " mass kg", lambda x: f"{x['mass']:8.2f}")
 
 
 def format_table(s: dict, max_traj_len: int) -> str:
@@ -342,17 +380,18 @@ def format_table(s: dict, max_traj_len: int) -> str:
 
 
 def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None,
-                     footsteps=None, delays=None) -> dict:
+                     footsteps=None, delays=None, payloads=None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
     out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
     push-recovery sweep, with its table and `summary.push`.  commands = [(mode name, value), ...]: the command-tracking sweep
     (env i holds the command of cell i mod len(commands)), with its table and `summary.commands`.  footsteps = [(plan type name,
     value), ...]: the footstep sweep (env i resets with the plan of cell i mod len(footsteps)), with its table and
     `summary.footsteps_sweep`.  delays = [seconds, ...]: the latency sweep (env i has the action delay of cell i mod len(delays)),
-    with its table and `summary.delay`.  Returns the report."""
-    if sum(x is not None for x in (push, commands, footsteps, delays)) > 1:
-        raise ValueError("the push, command, footstep and latency sweeps are separate evaluations")
-    sweep = held = plans = delay = None
+    with its table and `summary.delay`.  payloads = dict(masses=[kg, ...], at=(x, y, z)): the payload sweep (env i carries the
+    mass of cell i mod len(masses) at `at`), with its table and `summary.payload`.  Returns the report."""
+    if sum(x is not None for x in (push, commands, footsteps, delays, payloads)) > 1:
+        raise ValueError("the push, command, footstep, latency and payload sweeps are separate evaluations")
+    sweep = held = plans = delay = load = None
     if push is not None:
         k = int(round(push["push_at"] / env.dt))
         speed, dir_deg = push_grid(env.num_envs, push["speeds"], push["directions"])
@@ -365,7 +404,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         plans = (fs_mode, fs_value)
     if delays is not None:
         delay = delay_grid(env.num_envs, delays)
-    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans, delay=delay)
+    if payloads is not None:
+        load = payload_grid(env.num_envs, payloads["masses"])
+    out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans, delay=delay,
+                  payload=None if load is None else (load, payloads["at"]))
     acc, cacc = (out[0].cpu().numpy(), out[1].cpu().numpy()) if commands is not None else (out.cpu().numpy(), None)
     summary = summarize(acc, env.model_name, env.reward_names)
     pe = per_env(acc, env.model_name, env.reward_names)
@@ -388,6 +430,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         summary["delay"] = delay_summary(acc, delay, delays, env.model_name, env.reward_names)
         pe.update(action_delay=delay.tolist())
         print(format_delay_table(summary["delay"]))
+    if payloads is not None:
+        summary["payload"] = payload_summary(acc, load, payloads["masses"], payloads["at"], env.model_name, env.reward_names)
+        pe.update(payload_mass=load.tolist())
+        print(format_payload_table(summary["payload"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
                   max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:

@@ -30,9 +30,10 @@ from .snapshot import SnapshotError, plain_args
 from .storage import BatchData
 from .workers import DeviceRolloutWorker
 
-# per-env int32 tensors an env may own beside its records (None when off), which a snapshot shard then holds too: the name, what
-# it is and the training flag that turns it on
-_PER_ENV = {"stair_level": ("stair levels", "--stair-curriculum"), "action_delay": ("action delays", "--action-delay")}
+# per-env tensors an env may own beside its records (None when off), which a snapshot shard then holds too: the name, what it is
+# and the training flag that turns it on
+_PER_ENV = {"stair_level": ("stair levels", "--stair-curriculum"), "action_delay": ("action delays", "--action-delay"),
+            "payload": ("payloads", "--payload-mass")}
 
 
 class _FusedPPOLoss(torch.autograd.Function):

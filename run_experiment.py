@@ -80,6 +80,10 @@ TRAIN_FLAGS = [
                                                            "moved by each FORWARD episode (0: off, the reference's schedule; DESIGN §7.8)")),
     ("--action-delay", dict(type=_F, default=0.0, help="random action delays: every reset draws its env's delay uniformly from whole "
                                                        "physics substeps in [0, S] s, S <= control_dt (0: off; DESIGN §7.9)")),
+    ("--payload-mass", dict(type=_F, default=0.0, help="random payloads: every reset draws a point mass U(0, M) kg on its env's root "
+                                                       "link, M <= half the robot's mass (0: off; DESIGN §7.10)")),
+    ("--payload-offset", dict(type=_F, default=0.0, help="with --payload-mass: the payload's offset from the root link's centre of "
+                                                         "mass is drawn from U(-R, R)^3 m in the link's frame, R <= 0.25")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -107,7 +111,14 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
               # the latency sweep (DESIGN §7.9)
               ("--action-delays", dict(type=_S, default=None,
                                        help="comma-separated action delays in s, whole physics substeps up to control_dt, e.g. "
-                                            "0,0.005,0.01,0.02,0.025; with --num-envs one cell per delay, else exactly one"))]
+                                            "0,0.005,0.01,0.02,0.025; with --num-envs one cell per delay, else exactly one")),
+              # the payload sweep (DESIGN §7.10)
+              ("--payloads", dict(type=_S, default=None,
+                                  help="comma-separated payload masses in kg on the root link, at most half the robot's mass, e.g. "
+                                       "0,5,10,15,20; with --num-envs one cell per mass, else exactly one")),
+              ("--payload-at", dict(type=_S, default=None,
+                                    help="with --payloads: the payload's point x,y,z in m in the root link's frame, relative to its "
+                                         "centre of mass, each within 0.25 (default 0,0,0)"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -136,6 +147,9 @@ def print_system_info(args, training=True):
             print(f"Stair curriculum: levels of 0.01 m up to {stairs} m")
         delay = getattr(args, "action_delay", 0.0)
         print(f"Action delays: up to {delay * 1000:g} ms, drawn at every reset" if delay > 0 else "Action delays: off")
+        payload = getattr(args, "payload_mass", 0.0)
+        if payload:
+            print(f"Payloads: up to {payload:g} kg, offset up to {getattr(args, 'payload_offset', 0.0):g} m per axis, drawn at every reset")
     print("=" * 60)
 
 
@@ -185,7 +199,9 @@ def make_env_fn(args, rank, world, local):
                      max_traj_len=args.max_traj_len, path_to_yaml=args.yaml, push_vel=getattr(args, "push_vel", 0.0),
                      push_interval=getattr(args, "push_interval", 15.0),   # an experiment.pkl without them: no pushes
                      stair_curriculum=getattr(args, "stair_curriculum", 0.0),   # nor a stair curriculum
-                     action_delay=getattr(args, "action_delay", 0.0))   # nor action delays
+                     action_delay=getattr(args, "action_delay", 0.0),   # nor action delays
+                     payload_mass=getattr(args, "payload_mass", 0.0),   # nor payloads
+                     payload_offset=getattr(args, "payload_offset", 0.0))
     _env = env_fn()
     if not args.no_mirror:
         try:
@@ -252,15 +268,31 @@ def check_action_delay(args):
         raise SystemExit(f"train --action-delay {delay}: {e}")
 
 
+def check_payload_mass(args):
+    """Refuse random payload ranges the env would refuse (the mass against the model after --yaml), before any environment or run
+    directory exists."""
+    from learninghumanoidwalking_b200.envs.batched_env import check_payload_range
+    mass, offset = getattr(args, "payload_mass", 0.0), getattr(args, "payload_offset", 0.0)
+    try:
+        check_payload_range(mass, offset, _run_model(args.env, args.yaml)["total_mass"])
+    except ValueError as e:
+        raise SystemExit(f"train --payload-mass {mass} --payload-offset {offset}: {e}")
+
+
 def _run_cfg(env_name, yaml):
     """The model's cfg block after the user's YAML, as the env applies it."""
+    return _run_model(env_name, yaml)["cfg"]
+
+
+def _run_model(env_name, yaml):
+    """The model after the user's YAML, as the env applies it."""
     from learninghumanoidwalking_b200.model import load_model
     import_env(env_name)
     mj = load_model(env_name)
     if yaml is not None:
         from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
         mj = apply_config(mj, load_yaml(yaml))
-    return mj["cfg"]
+    return mj
 
 
 def run_experiment(args):
@@ -268,6 +300,7 @@ def run_experiment(args):
     check_push(args)
     check_stairs(args)
     check_action_delay(args)
+    check_payload_mass(args)
     rank, world, local = _dist_setup()
     timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
     args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
@@ -521,6 +554,50 @@ def check_delays(delays, run_args, yaml):
         raise SystemExit(f"eval --action-delays: {e}")
 
 
+def payload_cells(args):
+    """The payload masses of `eval --payloads ...` in kg and the one offset of --payload-at, or None without the flag; the
+    grammar, the offset and the combinations are refused here, the masses against the run's model by check_payloads."""
+    if args.payloads is None:
+        if args.payload_at is not None:
+            raise SystemExit("eval --payload-at places the payload of --payloads: add --payloads")
+        return None
+    try:
+        cells = [float(v) for v in args.payloads.split(",")]
+    except ValueError:
+        raise SystemExit(f"eval --payloads {args.payloads!r}: expected comma-separated masses in kg, e.g. 0,5,10,15,20")
+    if not all(v >= 0 and v < float("inf") for v in cells):
+        raise SystemExit(f"eval --payloads {args.payloads}: every mass must be finite and >= 0")
+    try:
+        at = [0.0, 0.0, 0.0] if args.payload_at is None else [float(v) for v in args.payload_at.split(",")]
+    except ValueError:
+        at = []
+    if len(at) != 3:
+        raise SystemExit(f"eval --payload-at {args.payload_at!r}: expected one point x,y,z in m, e.g. 0,0,0.1")
+    from learninghumanoidwalking_b200.envs.batched_env import PAYLOAD_MAX_OFFSET
+    if not all(abs(v) <= PAYLOAD_MAX_OFFSET for v in at):
+        raise SystemExit(f"eval --payload-at {args.payload_at}: every coordinate must be finite and within {PAYLOAD_MAX_OFFSET:g} m")
+    if (args.push_speeds is not None or args.command is not None or args.footsteps is not None
+            or args.action_delays is not None):
+        raise SystemExit("eval --payloads, --push-speeds, --command, --footsteps and --action-delays are separate sweeps: run them "
+                         "one at a time")
+    if args.num_envs is None and len(cells) != 1:
+        raise SystemExit(f"eval --payloads: {len(cells)} masses need the batched evaluation (add --num-envs N); the single-env "
+                         "roll-out takes exactly one")
+    if args.num_envs is not None and args.num_envs < len(cells):
+        raise SystemExit(f"eval --num-envs {args.num_envs}: --payloads lists {len(cells)} cells, and every cell needs at least one "
+                         "environment")
+    return dict(masses=cells, at=at)
+
+
+def check_payloads(payloads, run_args, yaml):
+    """Refuse masses the run's env would refuse (at most half its total_mass), before the actor is loaded."""
+    from learninghumanoidwalking_b200.envs.batched_env import check_payload
+    try:
+        check_payload(payloads["masses"], payloads["at"], _run_model(run_args.env, yaml)["total_mass"])
+    except ValueError as e:
+        raise SystemExit(f"eval --payloads: {e}")
+
+
 def check_footstep_env(env_name):
     """Refuse --footsteps for a run whose env is not jvrc_step, before its actor is loaded."""
     if env_name != "jvrc_step":
@@ -538,6 +615,7 @@ def evaluate_batched(args):
     commands = command_cells(args)
     footsteps = footstep_cells(args)
     delays = delay_cells(args)
+    payloads = payload_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -551,6 +629,8 @@ def evaluate_batched(args):
         yaml = str(Path(path_to_actor.parent, Path(yaml).name))      # the copy that rode along with the run, as `resume` uses
     if delays is not None:
         check_delays(delays, run_args, yaml)
+    if payloads is not None:
+        check_payloads(payloads, run_args, yaml)
     if push is not None:       # the push step needs the run's control step and horizon; refused before the actor is loaded
         from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
         from learninghumanoidwalking_b200.model import load_model
@@ -570,7 +650,7 @@ def evaluate_batched(args):
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
     report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands,
-                 footsteps=footsteps, delays=delays)
+                 footsteps=footsteps, delays=delays, payloads=payloads)
     env.close()
     return report
 
@@ -586,6 +666,7 @@ def evaluate(args):
     commands = command_cells(args)
     footsteps = footstep_cells(args)
     delays = delay_cells(args)
+    payloads = payload_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -596,6 +677,8 @@ def evaluate(args):
         check_footstep_env(run_args.env)
     if delays is not None:
         check_delays(delays, run_args, None)     # the single-env roll-out runs the env's own model, as it always has
+    if payloads is not None:
+        check_payloads(payloads, run_args, None)
     cv2 = None
     if args.out_dir is not None:
         try:
@@ -621,6 +704,8 @@ def evaluate(args):
             env.set_command(mode, command_refs(mode, value))
         if delays is not None:       # the one delay, set again after every reset
             env.set_action_delay(delays)
+        if payloads is not None:     # the one payload, set again after every reset (the video does not draw it)
+            env.set_payload(payloads["masses"], payloads["at"])
         return env.obs.float()
 
     obs = reset()
