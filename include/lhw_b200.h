@@ -196,6 +196,25 @@ int lhw_sim_step_payload(lhw_sim* sim, void* state_r, int32_t* state_i, int n_en
 int lhw_sim_draw_payload(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
                          double max_mass, double max_offset, void* payload, void* stream);
 
+/* lhw_sim_step_motor: lhw_sim_step with a motor strength per env and actuated joint (DESIGN.md §7.11), every variant.  strength
+ * [n][NU] (device, the sim's precision; NU = act_dim, in get_motor_names() order) holds each env's factors s_l >= 0, read once
+ * per control step: the step's PD gains become kp_step[l] = s_l kp, kd_step[l] = s_l kd (kp, kd after the pdrand_k draw when that
+ * is on), so the dynamics, act_force, the torque reward terms, prev_torque and H1's observed motor torques all see the scaled
+ * torque.  The substep loop and an auto-reset's settling (ctrl = 0) are unchanged.  An env whose factors are all exactly 1 is
+ * lhw_sim_step bit for bit; s_l = 0 leaves joint l limp.  payload [n][4] (or NULL for none) adds the payloads of
+ * lhw_sim_step_payload, delay [n] (device int32, or NULL for none) the action delays of lhw_sim_step_delay; level != NULL
+ * (jvrc_step only) adds the stair curriculum of lhw_sim_step_stairs, with its refusals.  Nothing writes strength, payload or delay.
+ * lhw_sim_draw_motor: the random strengths.  Every env whose mask [n] word is non-zero (every env when mask is NULL; pass the
+ * step's `ended`, or a reset's mask) gets strength[i][l] = 1 + max_dev (2 u01(u[l % 4]) - 1) with
+ * u = philox(seed, first_env_id + i, rng_ctr, 73 + l / 4), rng_ctr the record's event counter (state_i[i][4]) as the reset left
+ * it.  Only strength is written.  max_dev not finite or outside [0, 1] is refused with -2.  Reads no model constant but NU. */
+int lhw_sim_step_motor(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                       const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
+                       void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, const void* strength,
+                       const void* payload, const int32_t* delay, int32_t* level, int n_levels, void* stream);
+int lhw_sim_draw_motor(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
+                       double max_dev, void* strength, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

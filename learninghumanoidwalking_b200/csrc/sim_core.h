@@ -2292,12 +2292,15 @@ LHW_DEV int action_delay_clamp(int d, int frame_skip) { return d < 0 ? 0 : d > f
 // 0 .. delay-1 drive the PD loop towards the previous control step's target (prev_action, which holds it until the record update
 // below), the rest towards this step's; delay is already clamped to [0, frame_skip].  At delay 0 the step is the plain one.
 // PAYLOAD (DESIGN.md §7.10): every substep of the step builds the root link with the payload pay (root_payload); an auto-reset's
-// settling substeps do not.  A payload of mass 0 is the plain step
-template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false>
+// settling substeps do not.  A payload of mass 0 is the plain step.  MOTOR (DESIGN.md §7.11): strength[0 .. NU-1] holds the env's
+// per-joint motor strengths; the step's gains become kp_step[l] = s_l kp and kd_step[l] = s_l kd (kp, kd after the pdrand_k draw),
+// so the dynamics, act_force, the torque rewards, prev_torque and H1's observed torques all see the scaled torque.  Read once
+// per control step, here in the prologue; the substep loop is untouched.  Strength 1 is the plain step (kp 1 is exact)
+template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false, bool MOTOR = false>
 LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const real* action, uint32_t seed, int max_traj_len,
                       int autoreset, const int block_sync, const int alive, real* obs_out, real* term_obs_out, real* reward_out, real* rew_terms_out,
                       int32_t* done_out, int32_t* ended_out, int32_t* ep_len_out, real* ep_rew_out, int32_t* level = nullptr,
-                      int n_levels = 0, const int delay = 0, const Payload<real> pay = {}) {
+                      int n_levels = 0, const int delay = 0, const Payload<real> pay = {}, const real* strength = nullptr) {
   constexpr int NU = 2 * NJ, NOBS = Work<real, NJ, TK>::NOBS;
   // action smoothing + nominal offsets (base_humanoid_env.py:209-212, robot_base.py:80-85)
   // one event counter per control step: every draw of this step is keyed by rng_ctr + 1 (stored below)
@@ -2316,6 +2319,10 @@ LHW_DEV void env_step(Work<real, NJ, TK>& w, const Model<real, NJ, TK>& m, const
         philox(seed, w.env_id, w.rng_ctr + 1, 11 + (l >> 2), u);
         lo = (1 - m.pdrand_k) * kd; hi = (1 + m.pdrand_k) * kd;
         kd = lo + (hi - lo) * u01<real>(u[l & 3]);
+      }
+      if constexpr (MOTOR) {
+        const real s = strength[l];
+        kp = s * kp; kd = s * kd;
       }
       w.kp_step[l] = kp; w.kd_step[l] = kd;
     }
@@ -2661,7 +2668,7 @@ LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward,
 // The random pushes draw on their own Philox stream at the env's event counter, which they only read.  The step and reset
 // bodies above draw on streams 0-5, 8-13, 16-35, 40-48, 50-54 and 60-64, so with pushes off every trajectory is unchanged.
 // The random action delays draw on stream 71 (DELAY_STREAM, delay_draw_env below), the random payloads on stream 72
-// (PAYLOAD_STREAM, payload_draw_env below).
+// (PAYLOAD_STREAM, payload_draw_env below), the random motor strengths on streams 73-75 (MOTOR_STREAM, motor_draw_env below).
 constexpr uint32_t PUSH_STREAM = 70;
 
 // One env's push; returns 1 when it was pushed.  Explicit mode (d != nullptr): (dx, dy) = (d[0], d[1]), skipped when both are
@@ -2727,6 +2734,31 @@ LHW_DEV void payload_draw_env(const int32_t* si, uint32_t seed, uint32_t env_id,
   pay[0] = (real)(max_mass * u01<double>(u[0]));
 #pragma unroll
   for (int k = 0; k < 3; k++) pay[1 + k] = (real)(max_offset * (2 * u01<double>(u[1 + k]) - 1));
+}
+
+// ================================================================= random motor strengths (lhw_sim_draw_motor, DESIGN.md §7.11)
+// An env that was just reset (sel != 0: its ended word or mask word) draws the strengths of its new episode, one per actuated
+// joint l < nu: s_l = 1 + max_dev (2 u01(u) - 1) with u = philox(seed, env_id, rng_ctr, MOTOR_STREAM + l/4), lane l % 4, at the
+// event counter the reset left (si[4]), so s_l ~ U(1 - max_dev, 1 + max_dev).  The arithmetic is float64 at either precision,
+// rounded once to the strength's precision; the product and the sum are rounded separately on the device too (no fused
+// multiply-add), so the host body and numpy give the same bits.  Only out[0 .. nu-1] is written.
+constexpr uint32_t MOTOR_STREAM = 73;
+
+template <class real>
+LHW_DEV void motor_draw_env(const int32_t* si, uint32_t seed, uint32_t env_id, int32_t sel, double max_dev, int nu, real* out) {
+  if (!sel) return;
+  for (int b = 0; 4 * b < nu; b++) {
+    uint32_t u[4];
+    philox(seed, env_id, (uint32_t)si[4], MOTOR_STREAM + (uint32_t)b, u);
+    for (int k = 0; k < 4 && 4 * b + k < nu; k++) {
+      const double dev = max_dev * (2 * u01<double>(u[k]) - 1);
+#ifdef __CUDA_ARCH__
+      out[4 * b + k] = (real)__dadd_rn(1.0, dev);
+#else
+      out[4 * b + k] = (real)(1.0 + dev);
+#endif
+    }
+  }
 }
 
 // ================================================================= held commands (lhw_sim_set_command, DESIGN.md §7.6)

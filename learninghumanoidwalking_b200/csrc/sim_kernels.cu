@@ -131,15 +131,18 @@ __global__ void __launch_bounds__(32) reset_kernel(real* __restrict__ state_r, i
 // STAIRS (jvrc_step only, lhw_sim_step_stairs): level [n_envs] holds the envs' stair-curriculum levels of n_levels, moved and used
 // by the auto-resets (sim_core.h env_step).  DELAY (lhw_sim_step_delay): delay [n_envs] holds each env's action delay in substeps,
 // read once into a register and clamped to [0, frame_skip].  PAYLOAD (lhw_sim_step_payload, instantiated with DELAY): payload
-// [n_envs][4] holds each env's (m, rx, ry, rz), read once per control step; delay may then be null, which is delay 0
-template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false>
+// [n_envs][4] holds each env's (m, rx, ry, rz), read once per control step; delay may then be null, which is delay 0.  MOTOR
+// (lhw_sim_step_motor, instantiated with DELAY and PAYLOAD): strength [n_envs][NU] holds each env's per-joint motor strengths,
+// read once per control step; delay and payload may then be null, which is delay 0 and mass 0
+template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false, bool MOTOR = false>
 __global__ void __launch_bounds__(32, sizeof(real) == 4 ? (Cfg<NJ, TK>::SLABS ? 24 : 28) : (Cfg<NJ, TK>::SLABS ? 12 : (NJ == NJ_JVRC ? 16 : 15)))
     step_kernel(real* __restrict__ state_r, int32_t* __restrict__ state_i, int n_envs, uint32_t seed, uint32_t first_id,
                 const real* __restrict__ actions, int max_traj_len, int autoreset, real* __restrict__ obs,
                 real* __restrict__ term_obs, real* __restrict__ reward, real* __restrict__ rew_terms,
                 int32_t* __restrict__ done, int32_t* __restrict__ ended, int32_t* __restrict__ ep_len,
                 real* __restrict__ ep_rew, int32_t* __restrict__ level = nullptr, int n_levels = 0,
-                const int32_t* __restrict__ delay = nullptr, const real* __restrict__ payload = nullptr) {
+                const int32_t* __restrict__ delay = nullptr, const real* __restrict__ payload = nullptr,
+                const real* __restrict__ strength = nullptr) {
   using W = Work<real, NJ, TK>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int env = blockIdx.x;
@@ -152,18 +155,21 @@ __global__ void __launch_bounds__(32, sizeof(real) == 4 ? (Cfg<NJ, TK>::SLABS ? 
   load_state<real, NJ, TK>(w, sr, si, first_id + env);
   const int d = DELAY && (!PAYLOAD || delay) ? action_delay_clamp(delay[env], m.frame_skip) : 0;
   Payload<real> pl = {};
-  if constexpr (PAYLOAD) pl = {payload[4 * (size_t)env], {payload[4 * (size_t)env + 1], payload[4 * (size_t)env + 2], payload[4 * (size_t)env + 3]}};
-  env_step<real, NJ, TK, STAIRS, DELAY, PAYLOAD>(w, m, actions + (size_t)env * NU, seed, max_traj_len, autoreset, 0, 1, obs + (size_t)env * W::NOBS,
+  if constexpr (PAYLOAD) {
+    if (!MOTOR || payload) pl = {payload[4 * (size_t)env], {payload[4 * (size_t)env + 1], payload[4 * (size_t)env + 2], payload[4 * (size_t)env + 3]}};
+  }
+  env_step<real, NJ, TK, STAIRS, DELAY, PAYLOAD, MOTOR>(w, m, actions + (size_t)env * NU, seed, max_traj_len, autoreset, 0, 1, obs + (size_t)env * W::NOBS,
                      term_obs ? term_obs + (size_t)env * W::NOBS : nullptr, reward + env,
                      rew_terms ? rew_terms + (size_t)env * NREW : nullptr, done + env, ended + env,
-                     ep_len ? ep_len + env : nullptr, ep_rew ? ep_rew + env : nullptr, STAIRS ? level + env : nullptr, n_levels, d, pl);
+                     ep_len ? ep_len + env : nullptr, ep_rew ? ep_rew + env : nullptr, STAIRS ? level + env : nullptr, n_levels, d, pl,
+                     MOTOR ? strength + (size_t)env * NU : nullptr);
   store_state<real, NJ, TK>(w, sr, si);
 }
 
 // the shipped carving: W warps per block (one env each), a __syncthreads() per substep so the warps of an SM share
 // instruction-cache fills (far fewer no-instruction stalls); W from LHW_WARPS_PER_BLOCK or the defaults below.  STAIRS, DELAY,
-// PAYLOAD: as step_kernel
-template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false>
+// PAYLOAD, MOTOR: as step_kernel
+template <class real, int NJ, int TK, bool STAIRS = false, bool DELAY = false, bool PAYLOAD = false, bool MOTOR = false>
 // LHW_X_REGCAP (candidate, tools/ab_variants.py): the register budget of the fp64 lock-step kernel as "threads per SM" — 512 = 127
 // registers (16 warps per SM, the shipped kernel), 576 = 112 (18 warps), 640 = 96 (20 warps)
 #ifndef LHW_X_REGCAP
@@ -175,7 +181,8 @@ __global__ void __launch_bounds__(sizeof(real) == 8 ? LHW_X_REGCAP : 896, 1)
                    real* __restrict__ term_obs, real* __restrict__ reward, real* __restrict__ rew_terms,
                    int32_t* __restrict__ done, int32_t* __restrict__ ended, int32_t* __restrict__ ep_len,
                    real* __restrict__ ep_rew, int sync_mode, int32_t* __restrict__ level = nullptr, int n_levels = 0,
-                   const int32_t* __restrict__ delay = nullptr, const real* __restrict__ payload = nullptr) {
+                   const int32_t* __restrict__ delay = nullptr, const real* __restrict__ payload = nullptr,
+                   const real* __restrict__ strength = nullptr) {
   using W = Work<real, NJ, TK>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5;
@@ -190,11 +197,14 @@ __global__ void __launch_bounds__(sizeof(real) == 8 ? LHW_X_REGCAP : 896, 1)
   if (alive) load_state<real, NJ, TK>(w, sr, si, first_id + e);
   const int d = DELAY && (!PAYLOAD || delay) ? action_delay_clamp(delay[e], m.frame_skip) : 0;
   Payload<real> pl = {};
-  if constexpr (PAYLOAD) pl = {payload[4 * (size_t)e], {payload[4 * (size_t)e + 1], payload[4 * (size_t)e + 2], payload[4 * (size_t)e + 3]}};
-  env_step<real, NJ, TK, STAIRS, DELAY, PAYLOAD>(w, m, actions + (size_t)e * NU, seed, max_traj_len, autoreset, sync_mode, alive, obs + (size_t)e * W::NOBS,
+  if constexpr (PAYLOAD) {
+    if (!MOTOR || payload) pl = {payload[4 * (size_t)e], {payload[4 * (size_t)e + 1], payload[4 * (size_t)e + 2], payload[4 * (size_t)e + 3]}};
+  }
+  env_step<real, NJ, TK, STAIRS, DELAY, PAYLOAD, MOTOR>(w, m, actions + (size_t)e * NU, seed, max_traj_len, autoreset, sync_mode, alive, obs + (size_t)e * W::NOBS,
                      term_obs ? term_obs + (size_t)e * W::NOBS : nullptr, reward + e,
                      rew_terms ? rew_terms + (size_t)e * NREW : nullptr, done + e, ended + e,
-                     ep_len ? ep_len + e : nullptr, ep_rew ? ep_rew + e : nullptr, STAIRS ? level + e : nullptr, n_levels, d, pl);
+                     ep_len ? ep_len + e : nullptr, ep_rew ? ep_rew + e : nullptr, STAIRS ? level + e : nullptr, n_levels, d, pl,
+                     MOTOR ? strength + (size_t)e * NU : nullptr);
   if (alive) store_state<real, NJ, TK>(w, sr, si);
 }
 
@@ -242,6 +252,19 @@ __global__ void __launch_bounds__(256) payload_draw_kernel(const int32_t* __rest
   if (env >= n_envs) return;
   payload_draw_env<real>(state_i + (size_t)env * NSTATE_I, seed, first_id + env, mask ? mask[env] : 1, max_mass, max_offset,
                          payload + 4 * (size_t)env);
+}
+
+// random motor strengths: one thread per env, strength[i][0 .. nu-1] of the selected envs (mask[i] != 0, or every env without a
+// mask) redrawn, nothing else written (sim_core.h motor_draw_env); nu is an argument and no other model constant is read, so one
+// kernel per precision serves every variant
+template <class real>
+__global__ void __launch_bounds__(256) motor_draw_kernel(const int32_t* __restrict__ state_i, int n_envs, uint32_t seed,
+                                                        uint32_t first_id, const int32_t* __restrict__ mask, double max_dev, int nu,
+                                                        real* __restrict__ strength) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= n_envs) return;
+  motor_draw_env<real>(state_i + (size_t)env * NSTATE_I, seed, first_id + env, mask ? mask[env] : 1, max_dev, nu,
+                       strength + (size_t)nu * env);
 }
 
 // held commands (WalkingTask variants only): one thread per env, the mode word, mode_ref and the obs task words of the envs given
@@ -305,6 +328,10 @@ struct lhw_sim {
                             int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
                             int32_t* ended, int32_t* ep_len, void* ep_rew, const void* payload, const int32_t* delay, int32_t* level,
                             int n_levels, cudaStream_t st) = 0;
+  virtual void step_motor(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
+                          int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
+                          int32_t* ended, int32_t* ep_len, void* ep_rew, const void* strength, const void* payload,
+                          const int32_t* delay, int32_t* level, int n_levels, cudaStream_t st) = 0;
   virtual int frame_skip() const = 0;
   virtual void set_step_height(double h) = 0;
 };
@@ -350,6 +377,15 @@ template <class real, int NJ, int TK> int prepare_variant(lhw_sim* s) {
   if constexpr (Cfg<NJ, TK>::STEP) {
     if (prepare_kernel(step_kernel<real, NJ, TK, true, true, true>, s->work_bytes)) return -10;
     if (s->warps_per_block > 1 && prepare_kernel(step_kernel_mw<real, NJ, TK, true, true, true>, s->work_bytes * s->warps_per_block))
+      return -10;
+  }
+  if (prepare_kernel(step_kernel<real, NJ, TK, false, true, true, true>, s->work_bytes)) return -10;
+  if (s->warps_per_block > 1 && prepare_kernel(step_kernel_mw<real, NJ, TK, false, true, true, true>, s->work_bytes * s->warps_per_block))
+    return -10;
+  if constexpr (Cfg<NJ, TK>::STEP) {
+    if (prepare_kernel(step_kernel<real, NJ, TK, true, true, true, true>, s->work_bytes)) return -10;
+    if (s->warps_per_block > 1 &&
+        prepare_kernel(step_kernel_mw<real, NJ, TK, true, true, true, true>, s->work_bytes * s->warps_per_block))
       return -10;
   }
   return 0;
@@ -546,21 +582,41 @@ template <class real, int NJ, int TK> struct SimOf final : lhw_sim {
                                    reward, rew_terms, done, ended, ep_len, ep_rew, nullptr, 0, delay, st, payload);
   }
 
-  template <bool STAIRS, bool DELAY, bool PAYLOAD = false>
+  // MOTOR (with DELAY and PAYLOAD: a null delay array is delay 0, a null payload array mass 0), and with a level array (jvrc_step
+  // only) STAIRS as well
+  void step_motor(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
+                  int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
+                  int32_t* ended, int32_t* ep_len, void* ep_rew, const void* strength, const void* payload, const int32_t* delay,
+                  int32_t* level, int n_levels, cudaStream_t st) override {
+    if constexpr (Cfg<NJ, TK>::STEP) {
+      if (level) {
+        launch_step<true, true, true, true>(state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs,
+                                            term_obs, reward, rew_terms, done, ended, ep_len, ep_rew, level, n_levels, delay, st,
+                                            payload, strength);
+        return;
+      }
+    }
+    launch_step<false, true, true, true>(state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs, term_obs,
+                                         reward, rew_terms, done, ended, ep_len, ep_rew, nullptr, 0, delay, st, payload, strength);
+  }
+
+  template <bool STAIRS, bool DELAY, bool PAYLOAD = false, bool MOTOR = false>
   void launch_step(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const void* actions,
                    int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward, void* rew_terms, int32_t* done,
                    int32_t* ended, int32_t* ep_len, void* ep_rew, int32_t* level, int n_levels, const int32_t* delay, cudaStream_t st,
-                   const void* payload = nullptr) {
+                   const void* payload = nullptr, const void* strength = nullptr) {
     const int wpb = warps_per_block, grid = (n_envs + wpb - 1) / wpb;
     const size_t smem = work_bytes * wpb;
     if (wpb > 1)
-      step_kernel_mw<real, NJ, TK, STAIRS, DELAY, PAYLOAD><<<grid, wpb * 32, smem, st>>>(
+      step_kernel_mw<real, NJ, TK, STAIRS, DELAY, PAYLOAD, MOTOR><<<grid, wpb * 32, smem, st>>>(
           (real*)state_r, state_i, n_envs, seed, first_env_id, (const real*)actions, max_traj_len, autoreset, (real*)obs, (real*)term_obs,
-          (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew, sync_mode, level, n_levels, delay, (const real*)payload);
+          (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew, sync_mode, level, n_levels, delay, (const real*)payload,
+          (const real*)strength);
     else
-      step_kernel<real, NJ, TK, STAIRS, DELAY, PAYLOAD><<<grid, 32, smem, st>>>(
+      step_kernel<real, NJ, TK, STAIRS, DELAY, PAYLOAD, MOTOR><<<grid, 32, smem, st>>>(
           (real*)state_r, state_i, n_envs, seed, first_env_id, (const real*)actions, max_traj_len, autoreset, (real*)obs, (real*)term_obs,
-          (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew, level, n_levels, delay, (const real*)payload);
+          (real*)reward, (real*)rew_terms, done, ended, ep_len, (real*)ep_rew, level, n_levels, delay, (const real*)payload,
+          (const real*)strength);
   }
 
   int frame_skip() const override { return model.frame_skip; }
@@ -826,6 +882,42 @@ int lhw_sim_draw_payload(lhw_sim* s, const int32_t* state_i, int n_envs, uint32_
   else
     payload_draw_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(state_i, n_envs, seed, first_env_id, mask, max_mass, max_offset,
                                                                        (float*)payload);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_step_motor(lhw_sim* s, void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id,
+                       const void* actions, int max_traj_len, int autoreset, void* obs, void* term_obs, void* reward,
+                       void* rew_terms, int32_t* done, int32_t* ended, int32_t* ep_len, void* ep_rew, const void* strength,
+                       const void* payload, const int32_t* delay, int32_t* level, int n_levels, void* stream) {
+  if (!s || !state_r || !state_i || !actions || !obs || !reward || !done || !ended || !strength) return fail(-1, "null argument");
+  if (level) {
+    if (const int rc = check_stairs(s, n_levels, "lhw_sim_step_motor")) return rc;
+  }
+  if (n_envs <= 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (s->bind(st)) return -10;
+  s->step_motor(state_r, state_i, n_envs, seed, first_env_id, actions, max_traj_len, autoreset, obs, term_obs, reward, rew_terms,
+                done, ended, ep_len, ep_rew, strength, payload, delay, level, n_levels, st);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_draw_motor(lhw_sim* s, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
+                       double max_dev, void* strength, void* stream) {
+  if (!s || !state_i || !strength) return fail(-1, "null argument");
+  if (!(max_dev >= 0 && max_dev <= 1))
+    return fail(-2, "lhw_sim_draw_motor: the largest strength deviation must lie in [0, 1], got " + std::to_string(max_dev));
+  if (n_envs <= 0) return 0;
+  const int grid = (n_envs + 255) / 256;   // no model constants but the joint count
+  if (s->precision == 64)
+    motor_draw_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>(state_i, n_envs, seed, first_env_id, mask, max_dev, s->act_dim,
+                                                                      (double*)strength);
+  else
+    motor_draw_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(state_i, n_envs, seed, first_env_id, mask, max_dev, s->act_dim,
+                                                                     (float*)strength);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .sim_step_stairs, .sim_reset_stairs, .sim_step_delay, .sim_draw_delay, .sim_step_payload, .sim_draw_payload, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .sim_step_stairs, .sim_reset_stairs, .sim_step_delay, .sim_draw_delay, .sim_step_payload, .sim_draw_payload, .sim_step_motor, .sim_draw_motor, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -326,6 +326,45 @@ void sim_draw_payload(int64_t sim, const Tensor& state_i, int64_t seed, int64_t 
      "lhw_sim_draw_payload");
 }
 
+// the motor strengths (lhw_sim_step_motor / lhw_sim_draw_motor, DESIGN.md §7.11): strength [n, NU] of the sim's precision, the
+// factors of each env's actuated joints; the optional payload [n, 4], delay [n] int32 and level [n] int32 as sim_step_payload takes them
+void sim_step_motor(int64_t sim, Tensor state_r, Tensor state_i, int64_t seed, int64_t first_env_id, const Tensor& actions,
+                    int64_t max_traj_len, bool autoreset, Tensor obs, const OptTensor& term_obs, Tensor reward, const OptTensor& rew_terms,
+                    Tensor done, Tensor ended, const OptTensor& ep_len, const OptTensor& ep_rew, const Tensor& strength,
+                    const OptTensor& payload, const OptTensor& delay, const OptTensor& level, int64_t n_levels) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_r.dim() == 2, "lhw: state_r must be [n_envs, state_reals]");
+  const int64_t n = state_r.size(0);
+  check_step(I, state_r, state_i, actions, max_traj_len, obs, term_obs, reward, rew_terms, done, ended, ep_len, ep_rew);
+  check_cuda(strength, "strength", I.real, I.device); check_shape(strength, "strength", {n, I.nact});
+  if (payload) { check_cuda(*payload, "payload", I.real, I.device); check_shape(*payload, "payload", {n, 4}); }
+  if (delay) { check_cuda(*delay, "delay", at::kInt, I.device); check_shape(*delay, "delay", {n}); }
+  if (level) check_stairs(I, *level, n, n_levels);
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_step_motor(I.s, state_r.data_ptr(), state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                        actions.data_ptr(), (int)max_traj_len, autoreset ? 1 : 0, obs.data_ptr(), term_obs ? term_obs->data_ptr() : nullptr,
+                        reward.data_ptr(), rew_terms ? rew_terms->data_ptr() : nullptr, done.data_ptr<int32_t>(), ended.data_ptr<int32_t>(),
+                        ep_len ? ep_len->data_ptr<int32_t>() : nullptr, ep_rew ? ep_rew->data_ptr() : nullptr, strength.data_ptr(),
+                        payload ? payload->data_ptr() : nullptr, delay ? delay->data_ptr<int32_t>() : nullptr,
+                        level ? level->data_ptr<int32_t>() : nullptr, (int)n_levels, stream_of(state_r)),
+     "lhw_sim_step_motor");
+}
+
+// the largest deviation is checked by the C-ABI before its launch
+void sim_draw_motor(int64_t sim, const Tensor& state_i, int64_t seed, int64_t first_env_id, const OptTensor& mask, double max_dev,
+                    Tensor strength) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_i.dim() == 2, "lhw: state_i must be [n_envs, state_ints]");
+  const int64_t n = state_i.size(0);
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  check_cuda(strength, "strength", I.real, I.device); check_shape(strength, "strength", {n, I.nact});
+  if (mask) { check_cuda(*mask, "mask", at::kInt, I.device); check_shape(*mask, "mask", {n}); }
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_draw_motor(I.s, state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                        mask ? mask->data_ptr<int32_t>() : nullptr, max_dev, strength.data_ptr(), stream_of(state_i)),
+     "lhw_sim_draw_motor");
+}
+
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
          double gamma, double lam, const OptTensor& adv_partials) {
   TORCH_CHECK(rewards.dim() == 2, "lhw: rewards must be [T, N]");
@@ -547,6 +586,11 @@ TORCH_LIBRARY(lhw, m) {
         "Tensor(i!)? ep_len, Tensor(j!)? ep_rew, Tensor payload, Tensor? delay=None, Tensor(k!)? level=None, int n_levels=0) -> ()");
   m.def("sim_draw_payload(int sim, Tensor state_i, int seed, int first_env_id, Tensor? mask, float max_mass, float max_offset, "
         "Tensor(a!) payload) -> ()");
+  m.def("sim_step_motor(int sim, Tensor(a!) state_r, Tensor(b!) state_i, int seed, int first_env_id, Tensor actions, int max_traj_len, "
+        "bool autoreset, Tensor(c!) obs, Tensor(d!)? term_obs, Tensor(e!) reward, Tensor(f!)? rew_terms, Tensor(g!) done, Tensor(h!) ended, "
+        "Tensor(i!)? ep_len, Tensor(j!)? ep_rew, Tensor strength, Tensor? payload=None, Tensor? delay=None, Tensor(k!)? level=None, "
+        "int n_levels=0) -> ()");
+  m.def("sim_draw_motor(int sim, Tensor state_i, int seed, int first_env_id, Tensor? mask, float max_dev, Tensor(a!) strength) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -587,6 +631,8 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_draw_delay", &sim_draw_delay);
   m.impl("sim_step_payload", &sim_step_payload);
   m.impl("sim_draw_payload", &sim_draw_payload);
+  m.impl("sim_step_motor", &sim_step_motor);
+  m.impl("sim_draw_motor", &sim_draw_motor);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

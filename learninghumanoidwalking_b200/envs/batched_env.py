@@ -117,6 +117,26 @@ def check_payload_range(mass: float, offset: float, total_mass: float) -> None:
         raise ValueError("a payload offset range needs a payload mass range")
 
 
+MOTOR_STRENGTH_MAX = 2.0   # the largest motor strength a joint may be given (DESIGN.md §7.11)
+
+
+def check_motor_strength(strength) -> np.ndarray:
+    """Motor strength factors (a number or an array of any shape) as a float64 array of the same shape, after refusing a factor
+    that is not finite or lies outside [0, MOTOR_STRENGTH_MAX] (DESIGN.md §7.11)."""
+    s = np.asarray(strength, dtype=np.float64)
+    bad = ~np.isfinite(s) | (s < 0) | (s > MOTOR_STRENGTH_MAX)
+    if bad.any():
+        raise ValueError(f"a motor strength must lie in [0, {MOTOR_STRENGTH_MAX:g}], got {s[bad].reshape(-1)[0]}")
+    return s
+
+
+def check_motor_strength_range(max_dev: float) -> None:
+    """Refuse the random strengths' range R (every reset draws s ~ U(1 - R, 1 + R) per joint) unless it is finite and in [0, 1]."""
+    r = float(max_dev)
+    if not (0 <= r <= 1):
+        raise ValueError(f"a motor strength range must lie in [0, 1], got {max_dev}")
+
+
 class _Robot(SimpleNamespace):
     """The attributes the trainer reads / writes on `env.robot` (robots/robot_base.py:35, run_experiment.py:123-125).
     Writing `iteration_count` (rl/workers/rollout_worker.py:95) drives the SteppingTask's height curriculum."""
@@ -134,7 +154,7 @@ class BatchedHumanoidEnv:
                  domain_randomization: bool = True, init_noise: bool = True, pd_gain_randomization: float = 0.0,
                  iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0,
                  stair_curriculum: float = 0.0, action_delay: float = 0.0, payload_mass: float = 0.0,
-                 payload_offset: float = 0.0):
+                 payload_offset: float = 0.0, motor_strength: float = 0.0):
         # a stair level per env (DESIGN.md §7.8): every reset builds a FORWARD plan with its level's stair height, and each
         # auto-reset first moves the level by the ending FORWARD episode; off at 0, and then the launches are the plain ones
         self.stair_levels = stair_levels(model, stair_curriculum)
@@ -163,6 +183,9 @@ class BatchedHumanoidEnv:
         # U(-payload_offset, payload_offset)^3 on the root link
         check_payload_range(payload_mass, payload_offset, self.mj["total_mass"])
         self.payload_mass, self.payload_offset = float(payload_mass), float(payload_offset)
+        # random motor strengths (DESIGN.md §7.11): every reset draws its env's per-joint strengths from U(1 - R, 1 + R)
+        check_motor_strength_range(motor_strength)
+        self.motor_strength_range = float(motor_strength)
         if tolerance is None and precision == 32:
             tolerance = 1e-6  # fp32 cannot reach the reference's 1e-10; gradient floor is ~1e-6 of the force scale
         flat = pack_model(self.mj, tolerance=tolerance, max_iter=max_iter, observation_noise=observation_noise,
@@ -194,6 +217,9 @@ class BatchedHumanoidEnv:
         # [N, 4] of the env's dtype: each env's payload (m, rx, ry, rz); None (and the plain step kernels) until random payloads or
         # set_payload create it
         self.payload = torch.zeros(n, 4, dtype=self.dtype, device=dev) if self.payload_mass else None
+        # [N, act_dim] of the env's dtype: each env's motor strengths; None (and the launches without them) until random strengths
+        # or set_motor_strength create it
+        self.motor_strength = (torch.ones(n, self.act_dim, dtype=self.dtype, device=dev) if self.motor_strength_range else None)
         # ---- reference-facing attributes (envs/jvrc/jvrc_base.py:69-131, envs/jvrc/jvrc_walk.py:43-63)
         cfg = self.mj["cfg"]
         self.history_len = cfg["obs_history_len"]
@@ -276,6 +302,7 @@ class BatchedHumanoidEnv:
             self._fresh = False
         self._draw_delay(0, self.num_envs, mask)
         self._draw_payload(0, self.num_envs, mask)
+        self._draw_motor(0, self.num_envs, mask)
         return self.obs
 
     def step(self, actions: torch.Tensor, autoreset: bool = True):
@@ -283,6 +310,9 @@ class BatchedHumanoidEnv:
         With autoreset the RolloutWorker semantics apply (see include/lhw_b200.h: lhw_sim_step)."""
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
+        if self.motor_strength is not None:
+            self._step_motor(0, self.num_envs, actions, autoreset)
+            return self.obs, self.reward, self.done, self.ended
         if self.payload is not None:
             self._step_payload(0, self.num_envs, actions, autoreset)
             return self.obs, self.reward, self.done, self.ended
@@ -321,6 +351,9 @@ class BatchedHumanoidEnv:
         if actions.dtype != self.dtype or not actions.is_contiguous() or actions.device != self.device:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
         out = (self.obs[sl], self.reward[sl], self.done[sl], self.ended[sl])
+        if self.motor_strength is not None:
+            self._step_motor(lo, hi, actions, autoreset)
+            return out
         if self.payload is not None:
             self._step_payload(lo, hi, actions, autoreset)
             return out
@@ -424,6 +457,46 @@ class BatchedHumanoidEnv:
             self.payload = torch.zeros(self.num_envs, 4, dtype=self.dtype, device=self.device)
         self.payload.copy_(torch.from_numpy(host))
 
+    def _step_motor(self, lo: int, hi: int, actions: torch.Tensor, autoreset: bool) -> None:
+        """The control step of environments [lo, hi) with their motor strengths (and their payloads, action delays and stair levels
+        when those are on), then, with autoreset, the random draws of the envs it ended (and so reset), then the random pushes; all
+        on the current stream."""
+        sl = slice(lo, hi)
+        payload = None if self.payload is None else self.payload[sl]
+        delay = None if self.action_delay is None else self.action_delay[sl]
+        level = None if self.stair_level is None else self.stair_level[sl]
+        _lib.ops().sim_step_motor(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
+                                  self.max_traj_len, bool(autoreset), self.obs[sl], self.term_obs[sl], self.reward[sl], self.rew_terms[sl],
+                                  self.done[sl], self.ended[sl], self.ep_len[sl], self.ep_rew[sl], self.motor_strength[sl], payload, delay,
+                                  level, self.stair_levels)
+        if autoreset:
+            self._draw_delay(lo, hi, self.ended[sl])
+            self._draw_payload(lo, hi, self.ended[sl])
+            self._draw_motor(lo, hi, self.ended[sl])
+        self._push_random(lo, hi)
+
+    def _draw_motor(self, lo: int, hi: int, mask: torch.Tensor | None) -> None:
+        """Random mode: environments [lo, hi) whose mask word is non-zero (all without a mask), just reset, draw their new
+        episode's motor strengths; nothing is launched otherwise (include/lhw_b200.h: lhw_sim_draw_motor)."""
+        if self.motor_strength_range:
+            _lib.ops().sim_draw_motor(self._h.value, self.state_i[lo:hi], self.seed, self.first_env_id + lo, mask,
+                                      self.motor_strength_range, self.motor_strength[lo:hi])
+
+    def set_motor_strength(self, strength) -> None:
+        """Give every environment's actuated joints a motor strength: strength is [N, act_dim] (one factor per env and joint, in
+        get_motor_names() order) or [N] (one factor for all of an env's joints), each in [0, 2].  Joint l then delivers
+        s_l (kp (target - q) + kd (0 - qdot)).  The strengths hold until each env's next reset draws new ones (random mode,
+        motor_strength > 0) or until they are set again (include/lhw_b200.h: lhw_sim_step_motor)."""
+        s = torch.as_tensor(strength, dtype=torch.float64).detach().to("cpu")
+        if s.shape == (self.num_envs,):
+            s = s[:, None].expand(self.num_envs, self.act_dim)
+        if s.shape != (self.num_envs, self.act_dim):
+            raise ValueError(f"strength must be [{self.num_envs}, {self.act_dim}] or [{self.num_envs}], got {tuple(s.shape)}")
+        host = check_motor_strength(s.numpy())
+        if self.motor_strength is None:
+            self.motor_strength = torch.ones(self.num_envs, self.act_dim, dtype=self.dtype, device=self.device)
+        self.motor_strength.copy_(torch.from_numpy(np.ascontiguousarray(host)))
+
     def _push_random(self, lo: int, hi: int) -> None:
         """The random pushes of environments [lo, hi) after their control step, on the same stream; none at push_vel == 0.
         An env that the step ended (and so reset) is not pushed; the draws are keyed by the env's Philox id and event counter."""
@@ -500,10 +573,11 @@ class BatchedHumanoidEnv:
                                        mode.to(device=self.device, dtype=torch.int32), value.to(device=self.device, dtype=self.dtype),
                                        self._fresh, self.obs)
         self._fresh = False
-        if self.action_delay_max or self.payload_mass:
+        if self.action_delay_max or self.payload_mass or self.motor_strength_range:
             picked = (mode >= 0).to(device=self.device, dtype=torch.int32)
             self._draw_delay(0, self.num_envs, picked)
             self._draw_payload(0, self.num_envs, picked)
+            self._draw_motor(0, self.num_envs, picked)
         return self.obs
 
     def command_accumulate(self, acc: torch.Tensor) -> torch.Tensor:

@@ -28,6 +28,11 @@ The payload sweep (`eval --num-envs N --payloads 0,5,10,15,20 [--payload-at x,y,
 of cell i mod C, all at the one point --payload-at (BatchedHumanoidEnv.set_payload), after the reset, before the first step and
 outside the graph.  Autoreset is off, so nothing redraws it; the graph body is unchanged but for its step, which is the payload
 one.  Each cell's statistics are summarize()'s over its envs.
+
+The motor-strength sweep (`eval --num-envs N --motor-strengths 0,0.5,0.8,1,1.2 [--motor-joints R_KNEE,L_KNEE]`, DESIGN.md §7.11)
+gives env i the factor of cell i mod C on the named joints and 1 on the others (BatchedHumanoidEnv.set_motor_strength), after the
+reset, before the first step and outside the graph.  Autoreset is off, so nothing redraws them; the graph body is unchanged but for
+its step, which is the motor one.  Each cell's statistics are summarize()'s over its envs.
 """
 from __future__ import annotations
 
@@ -91,8 +96,14 @@ def payload_grid(n: int, masses) -> np.ndarray:
     return np.asarray(masses, dtype=np.float64)[np.arange(n) % len(masses)]
 
 
+def motor_grid(n: int, factors) -> np.ndarray:
+    """Per env the strength factor of the motor-strength sweep: env i is in cell i mod C of factors."""
+    return np.asarray(factors, dtype=np.float64)[np.arange(n) % len(factors)]
+
+
 @torch.no_grad()
-def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None, delay=None, payload=None):
+def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None, delay=None, payload=None,
+            motor=None):
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
     [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
     push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
@@ -101,7 +112,8 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None
     adds to the [N, C_WORDS] signed-velocity records; then the return is (accumulators, signed-velocity records).
     footsteps = (mode [N], value [N]): the reset is BatchedHumanoidEnv.reset_footsteps with these plans instead of reset().
     delay = seconds [N]: action delays (BatchedHumanoidEnv.set_action_delay) set after the reset.
-    payload = (mass [N], offset (x, y, z)): payloads (BatchedHumanoidEnv.set_payload) set after the reset."""
+    payload = (mass [N], offset (x, y, z)): payloads (BatchedHumanoidEnv.set_payload) set after the reset.
+    motor = strengths [N, act_dim]: motor strengths (BatchedHumanoidEnv.set_motor_strength) set after the reset."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
     if command is not None and env.command_words() != C_WORDS:
@@ -118,6 +130,8 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None
         env.set_action_delay(delay)
     if payload is not None:
         env.set_payload(*payload)
+    if motor is not None:
+        env.set_motor_strength(motor)
     state = env.obs.float().clone()
     push_k, push_d = push if push is not None else (None, None)
     if push is not None:
@@ -359,6 +373,18 @@ def format_payload_table(d: dict) -> str:
     return _format_cells(d, f"payloads at ({at}) m", " mass kg", lambda x: f"{x['mass']:8.2f}")
 
 
+def motor_summary(acc: np.ndarray, factor: np.ndarray, factors, joints, env_name: str, reward_names) -> dict:
+    """The motor-strength sweep's outcome per cell: the strength factor, n, and summarize()'s fall fraction, episode length,
+    return, per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the cell's envs; `joints`
+    are the joints that carry the factor, which every cell shares."""
+    return dict(factors=[float(f) for f in factors], joints=list(joints),
+                cells=_cell_summary(acc, factor, factors, "factor", env_name, reward_names))
+
+
+def format_motor_table(d: dict) -> str:
+    return _format_cells(d, f"motor strengths on {', '.join(d['joints'])}", "  factor", lambda x: f"{x['factor']:8.3f}")
+
+
 def format_table(s: dict, max_traj_len: int) -> str:
     L = s["length"]
     lines = [f"{s['num_envs']} environments, one episode each, horizon {max_traj_len} control steps",
@@ -380,7 +406,7 @@ def format_table(s: dict, max_traj_len: int) -> str:
 
 
 def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None,
-                     footsteps=None, delays=None, payloads=None) -> dict:
+                     footsteps=None, delays=None, payloads=None, motor=None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
     out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
     push-recovery sweep, with its table and `summary.push`.  commands = [(mode name, value), ...]: the command-tracking sweep
@@ -388,9 +414,11 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
     value), ...]: the footstep sweep (env i resets with the plan of cell i mod len(footsteps)), with its table and
     `summary.footsteps_sweep`.  delays = [seconds, ...]: the latency sweep (env i has the action delay of cell i mod len(delays)),
     with its table and `summary.delay`.  payloads = dict(masses=[kg, ...], at=(x, y, z)): the payload sweep (env i carries the
-    mass of cell i mod len(masses) at `at`), with its table and `summary.payload`.  Returns the report."""
-    if sum(x is not None for x in (push, commands, footsteps, delays, payloads)) > 1:
-        raise ValueError("the push, command, footstep, latency and payload sweeps are separate evaluations")
+    mass of cell i mod len(masses) at `at`), with its table and `summary.payload`.  motor = dict(factors=[...], joints=[names],
+    mask=[bool per joint]): the motor-strength sweep (env i's masked joints get the factor of cell i mod len(factors), the others 1),
+    with its table and `summary.motor_strength`.  Returns the report."""
+    if sum(x is not None for x in (push, commands, footsteps, delays, payloads, motor)) > 1:
+        raise ValueError("the push, command, footstep, latency, payload and motor-strength sweeps are separate evaluations")
     sweep = held = plans = delay = load = None
     if push is not None:
         k = int(round(push["push_at"] / env.dt))
@@ -406,8 +434,12 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         delay = delay_grid(env.num_envs, delays)
     if payloads is not None:
         load = payload_grid(env.num_envs, payloads["masses"])
+    strength = factor = None
+    if motor is not None:
+        factor = motor_grid(env.num_envs, motor["factors"])
+        strength = np.where(np.asarray(motor["mask"], dtype=bool)[None, :], factor[:, None], 1.0)
     out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans, delay=delay,
-                  payload=None if load is None else (load, payloads["at"]))
+                  payload=None if load is None else (load, payloads["at"]), motor=strength)
     acc, cacc = (out[0].cpu().numpy(), out[1].cpu().numpy()) if commands is not None else (out.cpu().numpy(), None)
     summary = summarize(acc, env.model_name, env.reward_names)
     pe = per_env(acc, env.model_name, env.reward_names)
@@ -434,6 +466,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         summary["payload"] = payload_summary(acc, load, payloads["masses"], payloads["at"], env.model_name, env.reward_names)
         pe.update(payload_mass=load.tolist())
         print(format_payload_table(summary["payload"]))
+    if motor is not None:
+        summary["motor_strength"] = motor_summary(acc, factor, motor["factors"], motor["joints"], env.model_name, env.reward_names)
+        pe.update(motor_strength=factor.tolist())
+        print(format_motor_table(summary["motor_strength"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
                   max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:

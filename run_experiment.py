@@ -84,6 +84,8 @@ TRAIN_FLAGS = [
                                                        "link, M <= half the robot's mass (0: off; DESIGN §7.10)")),
     ("--payload-offset", dict(type=_F, default=0.0, help="with --payload-mass: the payload's offset from the root link's centre of "
                                                          "mass is drawn from U(-R, R)^3 m in the link's frame, R <= 0.25")),
+    ("--motor-strength", dict(type=_F, default=0.0, help="random motor strengths: every reset draws each actuated joint's torque scale "
+                                                         "from U(1 - R, 1 + R), R in [0, 1] (0: off; DESIGN §7.11)")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -118,7 +120,14 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
                                        "0,5,10,15,20; with --num-envs one cell per mass, else exactly one")),
               ("--payload-at", dict(type=_S, default=None,
                                     help="with --payloads: the payload's point x,y,z in m in the root link's frame, relative to its "
-                                         "centre of mass, each within 0.25 (default 0,0,0)"))]
+                                         "centre of mass, each within 0.25 (default 0,0,0)")),
+              # the motor-strength sweep (DESIGN §7.11)
+              ("--motor-strengths", dict(type=_S, default=None,
+                                         help="comma-separated motor strength factors in [0, 2], e.g. 0,0.5,0.8,1,1.2; with --num-envs "
+                                              "one cell per factor, else exactly one")),
+              ("--motor-joints", dict(type=_S, default=None,
+                                      help="with --motor-strengths: comma-separated joint names (get_motor_names()) that get the factor, "
+                                           "e.g. R_KNEE,L_KNEE; the others keep 1 (default: every joint)"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -150,6 +159,9 @@ def print_system_info(args, training=True):
         payload = getattr(args, "payload_mass", 0.0)
         if payload:
             print(f"Payloads: up to {payload:g} kg, offset up to {getattr(args, 'payload_offset', 0.0):g} m per axis, drawn at every reset")
+        motor = getattr(args, "motor_strength", 0.0)
+        if motor:
+            print(f"Motor strengths: U({1 - motor:g}, {1 + motor:g}) per joint, drawn at every reset")
     print("=" * 60)
 
 
@@ -201,7 +213,8 @@ def make_env_fn(args, rank, world, local):
                      stair_curriculum=getattr(args, "stair_curriculum", 0.0),   # nor a stair curriculum
                      action_delay=getattr(args, "action_delay", 0.0),   # nor action delays
                      payload_mass=getattr(args, "payload_mass", 0.0),   # nor payloads
-                     payload_offset=getattr(args, "payload_offset", 0.0))
+                     payload_offset=getattr(args, "payload_offset", 0.0),
+                     motor_strength=getattr(args, "motor_strength", 0.0))   # nor motor strengths
     _env = env_fn()
     if not args.no_mirror:
         try:
@@ -279,6 +292,16 @@ def check_payload_mass(args):
         raise SystemExit(f"train --payload-mass {mass} --payload-offset {offset}: {e}")
 
 
+def check_motor_strength_flag(args):
+    """Refuse a random motor-strength range the env would refuse, before any environment or run directory exists."""
+    from learninghumanoidwalking_b200.envs.batched_env import check_motor_strength_range
+    r = getattr(args, "motor_strength", 0.0)
+    try:
+        check_motor_strength_range(r)
+    except ValueError as e:
+        raise SystemExit(f"train --motor-strength {r}: {e}")
+
+
 def _run_cfg(env_name, yaml):
     """The model's cfg block after the user's YAML, as the env applies it."""
     return _run_model(env_name, yaml)["cfg"]
@@ -301,6 +324,7 @@ def run_experiment(args):
     check_stairs(args)
     check_action_delay(args)
     check_payload_mass(args)
+    check_motor_strength_flag(args)
     rank, world, local = _dist_setup()
     timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
     args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
@@ -598,6 +622,55 @@ def check_payloads(payloads, run_args, yaml):
         raise SystemExit(f"eval --payloads: {e}")
 
 
+def motor_cells(args):
+    """The strength factors of `eval --motor-strengths ...` and the joint names of --motor-joints (None: every joint), or None
+    without the flag; the grammar, the range and the combinations are refused here, the joint names against the run's model by
+    motor_joint_mask."""
+    if args.motor_strengths is None:
+        if args.motor_joints is not None:
+            raise SystemExit("eval --motor-joints names the joints of --motor-strengths: add --motor-strengths")
+        return None
+    try:
+        cells = [float(v) for v in args.motor_strengths.split(",")]
+    except ValueError:
+        raise SystemExit(f"eval --motor-strengths {args.motor_strengths!r}: expected comma-separated factors, e.g. 0,0.5,0.8,1,1.2")
+    from learninghumanoidwalking_b200.envs.batched_env import check_motor_strength
+    try:
+        check_motor_strength(cells)
+    except ValueError as e:
+        raise SystemExit(f"eval --motor-strengths {args.motor_strengths}: {e}")
+    joints = None
+    if args.motor_joints is not None:
+        joints = [j.strip() for j in args.motor_joints.split(",")]
+        if not all(joints):
+            raise SystemExit(f"eval --motor-joints {args.motor_joints!r}: expected comma-separated joint names, e.g. R_KNEE,L_KNEE")
+    if (args.push_speeds is not None or args.command is not None or args.footsteps is not None
+            or args.action_delays is not None or args.payloads is not None):
+        raise SystemExit("eval --motor-strengths, --push-speeds, --command, --footsteps, --action-delays and --payloads are separate "
+                         "sweeps: run them one at a time")
+    if args.num_envs is None and len(cells) != 1:
+        raise SystemExit(f"eval --motor-strengths: {len(cells)} factors need the batched evaluation (add --num-envs N); the "
+                         "single-env roll-out takes exactly one")
+    if args.num_envs is not None and args.num_envs < len(cells):
+        raise SystemExit(f"eval --num-envs {args.num_envs}: --motor-strengths lists {len(cells)} cells, and every cell needs at "
+                         "least one environment")
+    return dict(factors=cells, joints=joints)
+
+
+def motor_joint_mask(motor, run_args, yaml):
+    """The [NU] bools of the joints --motor-joints names, in the run's model's joint order (every joint without the flag);
+    an unknown name is refused before the actor is loaded.  The joint names go into `motor` too."""
+    names = [lk["joint"]["name"] for lk in _run_model(run_args.env, yaml)["links"][1:]]
+    if motor["joints"] is None:
+        motor["joints"] = names
+    unknown = [j for j in motor["joints"] if j not in names]
+    if unknown:
+        raise SystemExit(f"eval --motor-joints: {', '.join(unknown)} is not a joint of the run's {run_args.env} model; its joints are "
+                         f"{', '.join(names)}")
+    motor["mask"] = [n in motor["joints"] for n in names]
+    return motor["mask"]
+
+
 def check_footstep_env(env_name):
     """Refuse --footsteps for a run whose env is not jvrc_step, before its actor is loaded."""
     if env_name != "jvrc_step":
@@ -616,6 +689,7 @@ def evaluate_batched(args):
     footsteps = footstep_cells(args)
     delays = delay_cells(args)
     payloads = payload_cells(args)
+    motor = motor_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -631,6 +705,8 @@ def evaluate_batched(args):
         check_delays(delays, run_args, yaml)
     if payloads is not None:
         check_payloads(payloads, run_args, yaml)
+    if motor is not None:
+        motor_joint_mask(motor, run_args, yaml)
     if push is not None:       # the push step needs the run's control step and horizon; refused before the actor is loaded
         from learninghumanoidwalking_b200.envs.config import apply_config, load_yaml
         from learninghumanoidwalking_b200.model import load_model
@@ -650,7 +726,7 @@ def evaluate_batched(args):
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
     report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands,
-                 footsteps=footsteps, delays=delays, payloads=payloads)
+                 footsteps=footsteps, delays=delays, payloads=payloads, motor=motor)
     env.close()
     return report
 
@@ -667,6 +743,7 @@ def evaluate(args):
     footsteps = footstep_cells(args)
     delays = delay_cells(args)
     payloads = payload_cells(args)
+    motor = motor_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -679,6 +756,8 @@ def evaluate(args):
         check_delays(delays, run_args, None)     # the single-env roll-out runs the env's own model, as it always has
     if payloads is not None:
         check_payloads(payloads, run_args, None)
+    if motor is not None:
+        motor_joint_mask(motor, run_args, None)
     cv2 = None
     if args.out_dir is not None:
         try:
@@ -706,6 +785,8 @@ def evaluate(args):
             env.set_action_delay(delays)
         if payloads is not None:     # the one payload, set again after every reset (the video does not draw it)
             env.set_payload(payloads["masses"], payloads["at"])
+        if motor is not None:        # the one strength on the named joints, set again after every reset
+            env.set_motor_strength([[motor["factors"][0] if on else 1.0 for on in motor["mask"]]])
         return env.obs.float()
 
     obs = reset()
