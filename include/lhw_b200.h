@@ -215,6 +215,25 @@ int lhw_sim_step_motor(lhw_sim* sim, void* state_r, int32_t* state_i, int n_envs
 int lhw_sim_draw_motor(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
                        double max_dev, void* strength, void* stream);
 
+/* lhw_sim_sense: sensor errors on the observations (DESIGN.md §7.12), every variant; a pass over obs (and term_obs) [n][obs_dim]
+ * after a step or a reset, on the same stream.  sensor [n][6 + NU] (device, the sim's precision) holds per env the noise
+ * multiplier m >= 0, then one offset per calibrated observation word: roll, pitch (rad), gyro x, y, z (rad/s) and the NU motor
+ * positions (rad, get_motor_names() order).  Word i < NROBOT (the robot-state words: 29 on JVRC-1, 35 on H1) of a treated
+ * observation x becomes (real)(x[i] + b_i + (m s_g) (2 u01(u[i % 4]) - 1)) in float64, b_i its offset (0 for velocities and
+ * torques), s_g its group's noise scale (orient 0.05, gyro 0.05, motor_pos 0.02, motor_vel 0.05, motor_tau 5) and
+ * u = philox(seed, first_env_id + i_env, rng_ctr, stream + i / 4) at the record's event counter (state_i[i_env][4]); a word with
+ * b_i == 0 and m s_g == 0 is not written.  The task words after NROBOT, the records and everything a step reads are never written.
+ * after_step != 0 (sel: the step's `ended`, term_obs required, else -2): with autoreset, an env that ended has its term_obs treated
+ * with its old row (stream 112), then draws (below), then its obs treated (stream 96); an env that did not end has its obs
+ * treated.  Without autoreset every obs is treated and term_obs gets the same words.  after_step == 0 (a reset; sel: its mask, or
+ * NULL for every env): a selected env draws, then its obs is treated; the others are not touched.  draw (host, {O, G, E}, or NULL
+ * for none): a drawing env's offsets become U(-O, O) for roll and pitch, U(-G, G) for the gyro, U(-E, E) for each motor position,
+ * offset k = (real)(r_k (2 u01(u[k % 4]) - 1)) with u = philox(seed, env id, rng_ctr, 80 + k / 4); the multiplier is never
+ * written.  O outside [0, 0.2], G outside [0, 0.5], E outside [0, 0.2] or not finite is refused with -2.  Reads no model constant
+ * but NROBOT, NU and obs_dim. */
+int lhw_sim_sense(lhw_sim* sim, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* sel,
+                  int after_step, int autoreset, const double* draw, void* sensor, void* obs, void* term_obs, void* stream);
+
 /* number of kernels this library has launched since load (the bench's gpu_launches claim) */
 long long lhw_launch_count(void);
 

@@ -58,6 +58,8 @@ SIGNATURES = {
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "lhw_sim_draw_motor": (c_int, [c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, ctypes.c_double, c_void_p, c_void_p]),
+    "lhw_sim_sense": (c_int, [c_void_p, c_void_p, c_int, c_uint32, c_uint32, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                              c_void_p, c_void_p]),
     "lhw_launch_count": (c_ll, []),
     "lhw_gae": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p,
                         c_void_p]),

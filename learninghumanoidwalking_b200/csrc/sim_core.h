@@ -2668,7 +2668,8 @@ LHW_DEV void eval_accumulate_env(const real* sr, const int32_t* si, real reward,
 // The random pushes draw on their own Philox stream at the env's event counter, which they only read.  The step and reset
 // bodies above draw on streams 0-5, 8-13, 16-35, 40-48, 50-54 and 60-64, so with pushes off every trajectory is unchanged.
 // The random action delays draw on stream 71 (DELAY_STREAM, delay_draw_env below), the random payloads on stream 72
-// (PAYLOAD_STREAM, payload_draw_env below), the random motor strengths on streams 73-75 (MOTOR_STREAM, motor_draw_env below).
+// (PAYLOAD_STREAM, payload_draw_env below), the random motor strengths on streams 73-75 (MOTOR_STREAM, motor_draw_env below), the
+// sensor errors on streams 80-84 (SENSOR_BIAS_STREAM), 96-104 (SENSOR_OBS_STREAM) and 112-120 (SENSOR_TERM_STREAM, sensor_env below).
 constexpr uint32_t PUSH_STREAM = 70;
 
 // One env's push; returns 1 when it was pushed.  Explicit mode (d != nullptr): (dx, dy) = (d[0], d[1]), skipped when both are
@@ -2759,6 +2760,93 @@ LHW_DEV void motor_draw_env(const int32_t* si, uint32_t seed, uint32_t env_id, i
 #endif
     }
   }
+}
+
+// ================================================================= sensor errors (lhw_sim_sense, DESIGN.md §7.12)
+// What the policy observes of the robot state, never what the step reads back: a pass over the observation rows after a step or a
+// reset.  An env's row [6 + nu] holds its noise multiplier m >= 0, then one offset per calibrated word: roll, pitch (rad), gyro
+// x, y, z (rad/s) and the nu motor positions (rad), i.e. obs word i < 5 + nu has offset row[1 + i]; velocity and torque words
+// have none.  Word i < nrobot of an observation x becomes
+//   x[i] = (real)((double)x[i] + b_i + (m s_g) (2 u01(u[i % 4]) - 1)),   u = philox(seed, env_id, rng_ctr, stream + i/4),
+// s_g the noise scale of word i's group (SENSOR_SCALE, the reference's H1 observation_noise.scales), rng_ctr the record's event
+// counter (si[4]).  Float64 at either precision, rounded once; the device rounds each product and sum on its own (no fused
+// multiply-add), so the host body and numpy give the same bits.  A word with b_i == 0 and m s_g == 0 is not written, so an
+// all-zero row leaves every bit of the observation, -0.0 included.  The task words after nrobot are never touched.
+constexpr uint32_t SENSOR_BIAS_STREAM = 80, SENSOR_OBS_STREAM = 96, SENSOR_TERM_STREAM = 112;
+// the noise scales s_g of the groups root_orient, root_ang_vel, motor_pos, motor_vel, motor_tau, for every robot (model/h1.json
+// cfg.observation_noise.scales)
+constexpr double SENSOR_SCALE_ORIENT = 0.05, SENSOR_SCALE_GYRO = 0.05, SENSOR_SCALE_POS = 0.02, SENSOR_SCALE_VEL = 0.05,
+                 SENSOR_SCALE_TAU = 5.0;
+// the largest noise multiplier, and the largest random (and explicit) roll / pitch, gyro and encoder offsets
+constexpr double SENSOR_MAX_NOISE = 4, SENSOR_MAX_ORIENT = 0.2, SENSOR_MAX_GYRO = 0.5, SENSOR_MAX_ENCODER = 0.2;
+
+LHW_DEV double sensor_fadd(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
+LHW_DEV double sensor_fmul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+
+// Words 4g .. 4g+3 (< nrobot) of one observation x with the row, on Philox stream `stream` (+ g); see above.
+template <class real>
+LHW_DEV void sensor_apply(const real* row, uint32_t seed, uint32_t env_id, uint32_t ctr, uint32_t stream, int g, int nrobot, int nu,
+                          real* x) {
+  uint32_t u[4];
+  philox(seed, env_id, ctr, stream + (uint32_t)g, u);
+  const double m = (double)row[0];
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int i = 4 * g + k;
+    const double b = i < 5 + nu ? (double)row[1 + i] : 0.0;
+    const double a = sensor_fmul(m, i < 2 ? SENSOR_SCALE_ORIENT : i < 5 ? SENSOR_SCALE_GYRO : i < 5 + nu ? SENSOR_SCALE_POS
+                                    : i < 5 + 2 * nu ? SENSOR_SCALE_VEL : SENSOR_SCALE_TAU);
+    if (i < nrobot && (b != 0 || a != 0))
+      x[i] = (real)sensor_fadd(sensor_fadd((double)x[i], b), sensor_fmul(a, 2 * u01<double>(u[k]) - 1));
+  }
+}
+
+// One env's group g of four observation words (g < ceil(nrobot / 4)): everything the pass does to those words, so no two calls
+// (threads) share a word and none needs another's result.  sel: the env's ended word after a step, its mask word (1 without a
+// mask) after a reset.
+//   after a step with autoreset, an ended env (sel != 0): term_obs gets the ending episode's row on SENSOR_TERM_STREAM; then, in
+//     random mode (draw != 0), the new episode's offsets are drawn; then obs (the new episode's first observation) gets the
+//     row on SENSOR_OBS_STREAM.  An env that did not end: obs only.
+//   after a step without autoreset: obs, and term_obs (which the step wrote equal to obs) gets the same words, so both stay equal.
+//   after a reset: a selected env draws (random mode) and its obs gets the row; an unselected env is not touched.
+// The draw (draw != 0, random mode): offset word k (row[1 + k], k < 5 + nu, the ones of this group: k = 4g .. 4g+3) =
+// (real)(r_k (2 u01(u[k % 4]) - 1)) with u = philox(seed, env_id, rng_ctr, SENSOR_BIAS_STREAM + k/4) and r_k = r_orient (roll,
+// pitch), r_gyro (gyro) or r_enc (motor positions); row[0], the multiplier, is never written.  rng_ctr is si[4] as the step's auto-reset or the reset left it.
+template <class real>
+LHW_DEV void sensor_env(const int32_t* si, uint32_t seed, uint32_t env_id, int g, int32_t sel, int after_step, int autoreset,
+                        int draw, double r_orient, double r_gyro, double r_enc, int nrobot, int nu, real* row, real* obs,
+                        real* term_obs) {
+  const uint32_t ctr = (uint32_t)si[4];
+  if (!after_step && !sel) return;
+  const bool new_episode = !after_step || (autoreset && sel);
+  if (after_step && new_episode) sensor_apply<real>(row, seed, env_id, ctr, SENSOR_TERM_STREAM, g, nrobot, nu, term_obs);
+  if (new_episode && draw) {
+    uint32_t u[4];
+    philox(seed, env_id, ctr, SENSOR_BIAS_STREAM + (uint32_t)g, u);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int k = 4 * g + j;
+      if (k < 5 + nu) row[1 + k] = (real)sensor_fmul(k < 2 ? r_orient : k < 5 ? r_gyro : r_enc, 2 * u01<double>(u[j]) - 1);
+    }
+  }
+  sensor_apply<real>(row, seed, env_id, ctr, SENSOR_OBS_STREAM, g, nrobot, nu, obs);
+  if (after_step && !autoreset)
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+      if (4 * g + k < nrobot) term_obs[4 * g + k] = obs[4 * g + k];
 }
 
 // ================================================================= held commands (lhw_sim_set_command, DESIGN.md §7.6)

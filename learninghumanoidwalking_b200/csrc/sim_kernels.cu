@@ -15,6 +15,7 @@
 #include <stdio.h>
 
 #include <atomic>
+#include <climits>
 #include <string>
 #include <vector>
 
@@ -267,6 +268,22 @@ __global__ void __launch_bounds__(256) motor_draw_kernel(const int32_t* __restri
                        strength + (size_t)nu * env);
 }
 
+// sensor errors: one thread per (env, group of four observation words), ngroup = ceil(nrobot / 4) threads per env (sim_core.h
+// sensor_env); nrobot, nu and obs_dim are arguments and no model constant is read, so one kernel per precision serves every variant
+template <class real>
+__global__ void __launch_bounds__(256) sensor_kernel(const int32_t* __restrict__ state_i, int n_envs, uint32_t seed, uint32_t first_id,
+                                                    const int32_t* __restrict__ sel, int after_step, int autoreset, double3 draw,
+                                                    int has_draw, int nrobot, int nu, int obs_dim, real* __restrict__ sensor,
+                                                    real* __restrict__ obs, real* __restrict__ term_obs) {
+  const int ngroup = (nrobot + 3) / 4;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;   // the host keeps n_envs * ngroup within int
+  if (t >= n_envs * ngroup) return;
+  const int env = t / ngroup, g = t - env * ngroup;
+  sensor_env<real>(state_i + (size_t)env * NSTATE_I, seed, first_id + env, g, sel ? sel[env] : 1, after_step, autoreset, has_draw,
+                   draw.x, draw.y, draw.z, nrobot, nu, sensor + (size_t)(6 + nu) * env, obs + (size_t)obs_dim * env,
+                   term_obs ? term_obs + (size_t)obs_dim * env : nullptr);
+}
+
 // held commands (WalkingTask variants only): one thread per env, the mode word, mode_ref and the obs task words of the envs given
 // one (sim_core.h set_command_env)
 template <class real, int NJ, int TK>
@@ -294,7 +311,7 @@ __global__ void __launch_bounds__(256) command_accumulate_kernel(const real* __r
 struct lhw_sim {
   int precision, device, warps_per_block, sync_mode;
   size_t work_bytes;
-  int state_reals, obs_dim, act_dim;
+  int state_reals, obs_dim, act_dim, nrobot;   // nrobot: the robot-state words that lead an observation
   virtual ~lhw_sim() = default;
   virtual int bind(cudaStream_t st) = 0;
   virtual void reset(void* state_r, int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* mask,
@@ -347,6 +364,7 @@ template <class real, int NJ, int TK> int prepare_variant(lhw_sim* s) {
   s->work_bytes = sizeof(Work<real, NJ, TK>);
   s->state_reals = Dims<real, NJ, TK>::NSTATE_R;
   s->obs_dim = Dims<real, NJ, TK>::NOBS;
+  s->nrobot = Dims<real, NJ, TK>::NROBOT;
   int maxsmem = 0;
   CUDA_OK(cudaDeviceGetAttribute(&maxsmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, s->device));
   // lock-step blocks: as many warps as the launch bound and the shared memory of one SM allow, two blocks per SM
@@ -918,6 +936,36 @@ int lhw_sim_draw_motor(lhw_sim* s, const int32_t* state_i, int n_envs, uint32_t 
   else
     motor_draw_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(state_i, n_envs, seed, first_env_id, mask, max_dev, s->act_dim,
                                                                      (float*)strength);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int lhw_sim_sense(lhw_sim* s, const int32_t* state_i, int n_envs, uint32_t seed, uint32_t first_env_id, const int32_t* sel,
+                  int after_step, int autoreset, const double* draw, void* sensor, void* obs, void* term_obs, void* stream) {
+  if (!s || !state_i || !sensor || !obs) return fail(-1, "null argument");
+  if (after_step && !term_obs) return fail(-2, "lhw_sim_sense: after a step the pass needs the step's term_obs");
+  if (draw) {
+    static const char* what[3] = {"roll / pitch offset", "gyro offset", "encoder offset"};
+    const double hi[3] = {SENSOR_MAX_ORIENT, SENSOR_MAX_GYRO, SENSOR_MAX_ENCODER};
+    for (int k = 0; k < 3; k++)
+      if (!(draw[k] >= 0 && draw[k] <= hi[k]))
+        return fail(-2, std::string("lhw_sim_sense: the largest ") + what[k] + " must lie in [0, " + std::to_string(hi[k]) + "], got " +
+                            std::to_string(draw[k]));
+  }
+  if (n_envs <= 0) return 0;
+  const long long threads = (long long)n_envs * ((s->nrobot + 3) / 4);
+  if (threads > INT_MAX) return fail(-2, "lhw_sim_sense: too many environments for one launch");
+  const int grid = (int)((threads + 255) / 256);   // no model constants but the three sizes
+  const double3 r = draw ? make_double3(draw[0], draw[1], draw[2]) : make_double3(0, 0, 0);
+  if (s->precision == 64)
+    sensor_kernel<double><<<grid, 256, 0, (cudaStream_t)stream>>>(state_i, n_envs, seed, first_env_id, sel, after_step, autoreset, r,
+                                                                  draw != nullptr, s->nrobot, s->act_dim, s->obs_dim, (double*)sensor,
+                                                                  (double*)obs, (double*)term_obs);
+  else
+    sensor_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(state_i, n_envs, seed, first_env_id, sel, after_step, autoreset, r,
+                                                                 draw != nullptr, s->nrobot, s->act_dim, s->obs_dim, (float*)sensor,
+                                                                 (float*)obs, (float*)term_obs);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -1,5 +1,5 @@
 // torch_ops.cpp — the entry points of include/lhw_b200.h registered with PyTorch's C++ extension ABI (TORCH_LIBRARY):
-// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .sim_step_stairs, .sim_reset_stairs, .sim_step_delay, .sim_draw_delay, .sim_step_payload, .sim_draw_payload, .sim_step_motor, .sim_draw_motor, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
+// torch.ops.lhw.sim_step(...), .sim_reset, .sim_render, .sim_eval_accumulate, .sim_push, .sim_set_command, .sim_command_accumulate, .sim_reset_footsteps, .sim_step_stairs, .sim_reset_stairs, .sim_step_delay, .sim_draw_delay, .sim_step_payload, .sim_draw_payload, .sim_step_motor, .sim_draw_motor, .sim_sense, .gae, .adv_stats, .adv_apply, .gather_minibatch, .grad_sumsq, .clip_adam_dev,
 // .fused_exchange, .fused_exchange_adaptive.  Thin: every op validates its tensors (device, dtype, contiguity, shape against the sim / comm
 // handle) with TORCH_CHECK, takes the CURRENT CUDA stream of the tensors' device and calls the C-ABI of liblhw_b200.so
 // underneath — a wrong-length or wrong-dtype tensor is an exception here instead of an out-of-bounds write in a kernel.
@@ -365,6 +365,28 @@ void sim_draw_motor(int64_t sim, const Tensor& state_i, int64_t seed, int64_t fi
      "lhw_sim_draw_motor");
 }
 
+// the sensor errors (lhw_sim_sense, DESIGN.md §7.12): sensor [n, 6 + NU] of the sim's precision; sel [n] int32 (the step's ended,
+// a reset's mask, or None for every env); term_obs is needed after a step; draw = [O, G, E] (random mode) or None, checked by the
+// C-ABI before its launch
+void sim_sense(int64_t sim, const Tensor& state_i, int64_t seed, int64_t first_env_id, const OptTensor& sel, bool after_step,
+               bool autoreset, std::optional<at::ArrayRef<double>> draw, Tensor sensor, Tensor obs, const OptTensor& term_obs) {
+  const SimInfo I = sim_info(sim);
+  TORCH_CHECK(state_i.dim() == 2, "lhw: state_i must be [n_envs, state_ints]");
+  const int64_t n = state_i.size(0);
+  check_cuda(state_i, "state_i", at::kInt, I.device); check_shape(state_i, "state_i", {n, I.ni});
+  check_cuda(sensor, "sensor", I.real, I.device); check_shape(sensor, "sensor", {n, 6 + I.nact});
+  check_cuda(obs, "obs", I.real, I.device); check_shape(obs, "obs", {n, I.nobs});
+  if (term_obs) { check_cuda(*term_obs, "term_obs", I.real, I.device); check_shape(*term_obs, "term_obs", {n, I.nobs}); }
+  TORCH_CHECK(!after_step || term_obs.has_value(), "lhw: sim_sense after a step needs the step's term_obs");
+  if (sel) { check_cuda(*sel, "sel", at::kInt, I.device); check_shape(*sel, "sel", {n}); }
+  TORCH_CHECK(!draw.has_value() || draw->size() == 3, "lhw: draw must be [O, G, E] (the largest orient, gyro and encoder offsets)");
+  c10::cuda::CUDAGuard guard(I.device);
+  ok(lhw_sim_sense(I.s, state_i.data_ptr<int32_t>(), (int)n, (uint32_t)seed, (uint32_t)first_env_id,
+                   sel ? sel->data_ptr<int32_t>() : nullptr, after_step ? 1 : 0, autoreset ? 1 : 0, draw.has_value() ? draw->data() : nullptr,
+                   sensor.data_ptr(), obs.data_ptr(), term_obs ? term_obs->data_ptr() : nullptr, stream_of(state_i)),
+     "lhw_sim_sense");
+}
+
 void gae(const Tensor& rewards, const Tensor& values, const Tensor& ended, const Tensor& boot, const Tensor& last_val, Tensor returns,
          double gamma, double lam, const OptTensor& adv_partials) {
   TORCH_CHECK(rewards.dim() == 2, "lhw: rewards must be [T, N]");
@@ -591,6 +613,8 @@ TORCH_LIBRARY(lhw, m) {
         "Tensor(i!)? ep_len, Tensor(j!)? ep_rew, Tensor strength, Tensor? payload=None, Tensor? delay=None, Tensor(k!)? level=None, "
         "int n_levels=0) -> ()");
   m.def("sim_draw_motor(int sim, Tensor state_i, int seed, int first_env_id, Tensor? mask, float max_dev, Tensor(a!) strength) -> ()");
+  m.def("sim_sense(int sim, Tensor state_i, int seed, int first_env_id, Tensor? sel, bool after_step, bool autoreset, float[]? draw, "
+        "Tensor(a!) sensor, Tensor(b!) obs, Tensor(c!)? term_obs) -> ()");
   m.def("gae(Tensor rewards, Tensor values, Tensor ended, Tensor boot, Tensor last_val, Tensor(a!) returns, float gamma, float lam, "
         "Tensor(b!)? adv_partials) -> ()");
   m.def("adv_stats_from_gae(Tensor adv_partials, int n_envs, Tensor(a!) stats) -> ()");
@@ -633,6 +657,7 @@ TORCH_LIBRARY_IMPL(lhw, CompositeExplicitAutograd, m) {
   m.impl("sim_draw_payload", &sim_draw_payload);
   m.impl("sim_step_motor", &sim_step_motor);
   m.impl("sim_draw_motor", &sim_draw_motor);
+  m.impl("sim_sense", &sim_sense);
   m.impl("gae", &gae);
   m.impl("adv_stats_from_gae", &adv_stats_from_gae);
   m.impl("adv_stats", &adv_stats);

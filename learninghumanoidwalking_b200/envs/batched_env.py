@@ -137,6 +137,58 @@ def check_motor_strength_range(max_dev: float) -> None:
         raise ValueError(f"a motor strength range must lie in [0, 1], got {max_dev}")
 
 
+# sensor errors (DESIGN.md §7.12, csrc/sim_core.h SENSOR_MAX_*): the largest noise multiplier, and the largest roll / pitch (rad),
+# gyro (rad/s) and encoder (rad) offsets
+SENSOR_MAX_NOISE = 4.0
+SENSOR_MAX_BIAS = (0.2, 0.5, 0.2)
+SENSOR_BIAS_GROUPS = ("roll / pitch", "gyro", "encoder")
+
+
+def sensor_bias_bounds(nu: int) -> np.ndarray:
+    """The [5 + nu] bounds of an env's offsets, in the order of its sensor row after the multiplier: roll, pitch, gyro x, y, z,
+    then the nu motor positions."""
+    return np.repeat(np.asarray(SENSOR_MAX_BIAS), [2, 3, nu])
+
+
+def check_sensor_noise(noise) -> np.ndarray:
+    """Noise multipliers (a number or an array of any shape) as a float64 array of the same shape, after refusing one that is not
+    finite or lies outside [0, SENSOR_MAX_NOISE] (DESIGN.md §7.12)."""
+    m = np.asarray(noise, dtype=np.float64)
+    bad = ~np.isfinite(m) | (m < 0) | (m > SENSOR_MAX_NOISE)
+    if bad.any():
+        raise ValueError(f"a sensor noise multiplier must lie in [0, {SENSOR_MAX_NOISE:g}], got {m[bad].reshape(-1)[0]}")
+    return m
+
+
+def check_sensor_bias(bias, nu: int) -> np.ndarray:
+    """Sensor offsets [..., 5 + nu] (roll, pitch, gyro x, y, z, the nu motor positions) as a float64 array, after refusing one that
+    is not finite or whose magnitude is above its group's bound of SENSOR_MAX_BIAS."""
+    b = np.asarray(bias, dtype=np.float64)
+    if b.ndim == 0 or b.shape[-1] != 5 + nu:
+        raise ValueError(f"sensor offsets must hold 5 + {nu} = {5 + nu} words per env, got {tuple(b.shape)}")
+    bound = sensor_bias_bounds(nu)
+    bad = ~np.isfinite(b) | (np.abs(b) > bound)
+    if bad.any():
+        k = int(np.argwhere(bad)[0][-1])
+        g = 0 if k < 2 else 1 if k < 5 else 2
+        raise ValueError(f"a {SENSOR_BIAS_GROUPS[g]} offset must lie in [-{SENSOR_MAX_BIAS[g]:g}, {SENSOR_MAX_BIAS[g]:g}], "
+                         f"got {b[bad].reshape(-1)[0]}")
+    return b
+
+
+def check_sensor_range(noise: float, bias) -> tuple[float, tuple[float, float, float]]:
+    """The random sensor errors' multiplier M and offset ranges (O, G, E) as numbers, after refusing an M that check_sensor_noise
+    refuses, a bias that is not three numbers, and a range that is not finite or lies outside [0, its SENSOR_MAX_BIAS bound]."""
+    m = float(check_sensor_noise(float(noise)))
+    b = np.asarray(bias, dtype=np.float64).reshape(-1)
+    if b.shape != (3,):
+        raise ValueError(f"a sensor bias range must be three numbers O, G, E (roll / pitch, gyro, encoder), got {bias}")
+    for g in range(3):
+        if not (0 <= b[g] <= SENSOR_MAX_BIAS[g]):
+            raise ValueError(f"a {SENSOR_BIAS_GROUPS[g]} offset range must lie in [0, {SENSOR_MAX_BIAS[g]:g}], got {b[g]}")
+    return m, (float(b[0]), float(b[1]), float(b[2]))
+
+
 class _Robot(SimpleNamespace):
     """The attributes the trainer reads / writes on `env.robot` (robots/robot_base.py:35, run_experiment.py:123-125).
     Writing `iteration_count` (rl/workers/rollout_worker.py:95) drives the SteppingTask's height curriculum."""
@@ -154,7 +206,8 @@ class BatchedHumanoidEnv:
                  domain_randomization: bool = True, init_noise: bool = True, pd_gain_randomization: float = 0.0,
                  iteration_count: float = float("inf"), path_to_yaml=None, push_vel: float = 0.0, push_interval: float = 15.0,
                  stair_curriculum: float = 0.0, action_delay: float = 0.0, payload_mass: float = 0.0,
-                 payload_offset: float = 0.0, motor_strength: float = 0.0):
+                 payload_offset: float = 0.0, motor_strength: float = 0.0, sensor_noise: float = 0.0,
+                 sensor_bias=(0.0, 0.0, 0.0)):
         # a stair level per env (DESIGN.md §7.8): every reset builds a FORWARD plan with its level's stair height, and each
         # auto-reset first moves the level by the ending FORWARD episode; off at 0, and then the launches are the plain ones
         self.stair_levels = stair_levels(model, stair_curriculum)
@@ -186,6 +239,9 @@ class BatchedHumanoidEnv:
         # random motor strengths (DESIGN.md §7.11): every reset draws its env's per-joint strengths from U(1 - R, 1 + R)
         check_motor_strength_range(motor_strength)
         self.motor_strength_range = float(motor_strength)
+        # random sensor errors (DESIGN.md §7.12): every env observes with noise multiplier sensor_noise, and every reset draws its
+        # offsets from U(-O, O) (roll, pitch), U(-G, G) (gyro), U(-E, E) (encoders), sensor_bias = (O, G, E)
+        self.sensor_noise, self.sensor_bias = check_sensor_range(sensor_noise, sensor_bias)
         if tolerance is None and precision == 32:
             tolerance = 1e-6  # fp32 cannot reach the reference's 1e-10; gradient floor is ~1e-6 of the force scale
         flat = pack_model(self.mj, tolerance=tolerance, max_iter=max_iter, observation_noise=observation_noise,
@@ -220,6 +276,12 @@ class BatchedHumanoidEnv:
         # [N, act_dim] of the env's dtype: each env's motor strengths; None (and the launches without them) until random strengths
         # or set_motor_strength create it
         self.motor_strength = (torch.ones(n, self.act_dim, dtype=self.dtype, device=dev) if self.motor_strength_range else None)
+        # [N, 6 + act_dim] of the env's dtype: each env's noise multiplier, then its offsets (roll, pitch, gyro x, y, z, the motor
+        # positions); None (and no sensor pass) until random sensor errors or set_sensor_errors create it
+        self.sensor = None
+        if self.sensor_noise or any(self.sensor_bias):
+            self.sensor = torch.zeros(n, 6 + self.act_dim, dtype=self.dtype, device=dev)
+            self.sensor[:, 0] = self.sensor_noise
         # ---- reference-facing attributes (envs/jvrc/jvrc_base.py:69-131, envs/jvrc/jvrc_walk.py:43-63)
         cfg = self.mj["cfg"]
         self.history_len = cfg["obs_history_len"]
@@ -303,6 +365,7 @@ class BatchedHumanoidEnv:
         self._draw_delay(0, self.num_envs, mask)
         self._draw_payload(0, self.num_envs, mask)
         self._draw_motor(0, self.num_envs, mask)
+        self._sense(0, self.num_envs, mask, False, False)
         return self.obs
 
     def step(self, actions: torch.Tensor, autoreset: bool = True):
@@ -312,24 +375,29 @@ class BatchedHumanoidEnv:
             actions = actions.to(device=self.device, dtype=self.dtype).contiguous()
         if self.motor_strength is not None:
             self._step_motor(0, self.num_envs, actions, autoreset)
+            self._sense(0, self.num_envs, self.ended, True, autoreset)
             return self.obs, self.reward, self.done, self.ended
         if self.payload is not None:
             self._step_payload(0, self.num_envs, actions, autoreset)
+            self._sense(0, self.num_envs, self.ended, True, autoreset)
             return self.obs, self.reward, self.done, self.ended
         if self.action_delay is not None:
             self._step_delay(0, self.num_envs, actions, autoreset)
+            self._sense(0, self.num_envs, self.ended, True, autoreset)
             return self.obs, self.reward, self.done, self.ended
         if self.stair_level is not None:
             _lib.ops().sim_step_stairs(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, actions, self.max_traj_len,
                                        bool(autoreset), self.obs, self.term_obs, self.reward, self.rew_terms, self.done, self.ended,
                                        self.ep_len, self.ep_rew, self.stair_level, self.stair_levels)
             self._push_random(0, self.num_envs)
+            self._sense(0, self.num_envs, self.ended, True, autoreset)
             return self.obs, self.reward, self.done, self.ended
         if _lib.use_torch_ops():     # torch.ops.lhw.sim_step: device / dtype / shape checks, then the C-ABI launch
             _lib.ops().sim_step(self._h.value, self.state_r, self.state_i, self.seed, self.first_env_id, actions, self.max_traj_len,
                                 bool(autoreset), self.obs, self.term_obs, self.reward, self.rew_terms, self.done, self.ended,
                                 self.ep_len, self.ep_rew)
             self._push_random(0, self.num_envs)
+            self._sense(0, self.num_envs, self.ended, True, autoreset)
             return self.obs, self.reward, self.done, self.ended
         assert actions.shape == (self.num_envs, self.act_dim), actions.shape
         L = _lib.lib()
@@ -341,6 +409,7 @@ class BatchedHumanoidEnv:
                                       self.ep_len.data_ptr(), self.ep_rew.data_ptr(), _lib.current_stream_ptr()),
                        "lhw_sim_step")
         self._push_random(0, self.num_envs)
+        self._sense(0, self.num_envs, self.ended, True, autoreset)
         return self.obs, self.reward, self.done, self.ended
 
     def step_slice(self, lo: int, hi: int, actions: torch.Tensor, autoreset: bool = True):
@@ -353,24 +422,29 @@ class BatchedHumanoidEnv:
         out = (self.obs[sl], self.reward[sl], self.done[sl], self.ended[sl])
         if self.motor_strength is not None:
             self._step_motor(lo, hi, actions, autoreset)
+            self._sense(lo, hi, out[3], True, autoreset)
             return out
         if self.payload is not None:
             self._step_payload(lo, hi, actions, autoreset)
+            self._sense(lo, hi, out[3], True, autoreset)
             return out
         if self.action_delay is not None:
             self._step_delay(lo, hi, actions, autoreset)
+            self._sense(lo, hi, out[3], True, autoreset)
             return out
         if self.stair_level is not None:
             _lib.ops().sim_step_stairs(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
                                        self.max_traj_len, bool(autoreset), out[0], self.term_obs[sl], out[1], self.rew_terms[sl], out[2],
                                        out[3], self.ep_len[sl], self.ep_rew[sl], self.stair_level[sl], self.stair_levels)
             self._push_random(lo, hi)
+            self._sense(lo, hi, out[3], True, autoreset)
             return out
         if _lib.use_torch_ops():
             _lib.ops().sim_step(self._h.value, self.state_r[sl], self.state_i[sl], self.seed, self.first_env_id + lo, actions,
                                 self.max_traj_len, bool(autoreset), out[0], self.term_obs[sl], out[1], self.rew_terms[sl], out[2], out[3],
                                 self.ep_len[sl], self.ep_rew[sl])
             self._push_random(lo, hi)
+            self._sense(lo, hi, out[3], True, autoreset)
             return out
         assert actions.shape == (hi - lo, self.act_dim), actions.shape
         with torch.cuda.device(self.device):
@@ -381,6 +455,7 @@ class BatchedHumanoidEnv:
                                                self.ep_len[sl].data_ptr(), self.ep_rew[sl].data_ptr(), _lib.current_stream_ptr()),
                        "lhw_sim_step")
         self._push_random(lo, hi)
+        self._sense(lo, hi, out[3], True, autoreset)
         return out
 
     def _step_delay(self, lo: int, hi: int, actions: torch.Tensor, autoreset: bool) -> None:
@@ -497,6 +572,41 @@ class BatchedHumanoidEnv:
             self.motor_strength = torch.ones(self.num_envs, self.act_dim, dtype=self.dtype, device=self.device)
         self.motor_strength.copy_(torch.from_numpy(np.ascontiguousarray(host)))
 
+    def _sense(self, lo: int, hi: int, sel: torch.Tensor | None, after_step: bool, autoreset: bool) -> None:
+        """The sensor errors of environments [lo, hi), on the current stream after the launches that wrote their observations;
+        nothing is launched while self.sensor is None.  After a step (sel: its ended flags), with autoreset an env that ended gets
+        the ending episode's errors on its term_obs, draws its new offsets (random mode) and gets them on its obs; every other obs
+        gets its env's errors, and without autoreset term_obs the same.  After a reset (sel: its mask, None for every env) the
+        selected envs draw (random mode) and get them on their obs (include/lhw_b200.h: lhw_sim_sense)."""
+        if self.sensor is None:
+            return
+        draw = list(self.sensor_bias) if any(self.sensor_bias) else None
+        _lib.ops().sim_sense(self._h.value, self.state_i[lo:hi], self.seed, self.first_env_id + lo, sel, bool(after_step),
+                             bool(autoreset), draw, self.sensor[lo:hi], self.obs[lo:hi], self.term_obs[lo:hi] if after_step else None)
+
+    def set_sensor_errors(self, noise, bias=None) -> None:
+        """Give every environment sensor errors: noise is one multiplier m or N of them, in [0, 4]; bias None (no offsets), one row
+        of 5 + act_dim offsets for every env or [N, 5 + act_dim]: roll and pitch (rad, at most 0.2), gyro x, y, z (rad/s, at most
+        0.5) and one per motor position (rad, at most 0.2, in get_motor_names() order).  Each observed robot-state word then gets
+        its offset plus m times its group's noise scale times U(-1, 1).  The errors hold until each env's next random draw (random
+        mode) or until they are set again; the current obs is not rewritten, so errors set before a reset apply from that reset's
+        observation on (include/lhw_b200.h: lhw_sim_sense)."""
+        n, nb = self.num_envs, 5 + self.act_dim
+        m = torch.as_tensor(noise, dtype=torch.float64).detach().to("cpu").reshape(-1)
+        if m.shape == (1,):
+            m = m.expand(n)
+        if m.shape != (n,):
+            raise ValueError(f"noise must be one number or {n}, got {tuple(m.shape)}")
+        b = np.zeros((n, nb)) if bias is None else torch.as_tensor(bias, dtype=torch.float64).detach().to("cpu").numpy()
+        if b.shape == (nb,):
+            b = np.broadcast_to(b, (n, nb))
+        if b.shape != (n, nb):
+            raise ValueError(f"bias must be None, [{nb}] or [{n}, {nb}], got {tuple(b.shape)}")
+        host = np.concatenate([check_sensor_noise(m.numpy())[:, None], check_sensor_bias(b, self.act_dim)], axis=1)
+        if self.sensor is None:
+            self.sensor = torch.zeros(n, 6 + self.act_dim, dtype=self.dtype, device=self.device)
+        self.sensor.copy_(torch.from_numpy(host))
+
     def _push_random(self, lo: int, hi: int) -> None:
         """The random pushes of environments [lo, hi) after their control step, on the same stream; none at push_vel == 0.
         An env that the step ended (and so reset) is not pushed; the draws are keyed by the env's Philox id and event counter."""
@@ -578,6 +688,8 @@ class BatchedHumanoidEnv:
             self._draw_delay(0, self.num_envs, picked)
             self._draw_payload(0, self.num_envs, picked)
             self._draw_motor(0, self.num_envs, picked)
+        if self.sensor is not None:
+            self._sense(0, self.num_envs, (mode >= 0).to(device=self.device, dtype=torch.int32), False, False)
         return self.obs
 
     def command_accumulate(self, acc: torch.Tensor) -> torch.Tensor:

@@ -33,6 +33,13 @@ The motor-strength sweep (`eval --num-envs N --motor-strengths 0,0.5,0.8,1,1.2 [
 gives env i the factor of cell i mod C on the named joints and 1 on the others (BatchedHumanoidEnv.set_motor_strength), after the
 reset, before the first step and outside the graph.  Autoreset is off, so nothing redraws them; the graph body is unchanged but for
 its step, which is the motor one.  Each cell's statistics are summarize()'s over its envs.
+
+The sensor sweep (`eval --num-envs N --sensor-errors roll:-0.05,0.05 pitch:0.1 encoder:0.03 noise:1,2`, DESIGN.md §7.12) gives
+env i the sensor errors of cell i mod C (BatchedHumanoidEnv.set_sensor_errors) before the reset, because the first observation
+is a sensor reading too: a roll or pitch cell sets that IMU offset, an encoder cell every motor-position offset, a noise cell the
+noise multiplier, and every other word of the cell is 0.  Autoreset is off, so nothing redraws them; the graph body is unchanged
+but for the sensor pass after its step.  Cells are (kind, value) pairs, so each cell's statistics are summarize()'s over the envs
+of its index.
 """
 from __future__ import annotations
 
@@ -101,9 +108,31 @@ def motor_grid(n: int, factors) -> np.ndarray:
     return np.asarray(factors, dtype=np.float64)[np.arange(n) % len(factors)]
 
 
+SENSOR_KINDS = ("roll", "pitch", "encoder", "noise")
+
+
+def sensor_grid(n: int, cells, nu: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The sensor sweep's rows: per env its cell index (env i is in cell i mod C of cells = [(kind, value), ...]), noise
+    multiplier [n] and offsets [n, 5 + nu] (roll, pitch, gyro x, y, z, the motor positions), 0 but for the cell's one kind."""
+    m, b = np.zeros(len(cells)), np.zeros((len(cells), 5 + nu))
+    for c, (kind, v) in enumerate(cells):
+        if kind == "roll":
+            b[c, 0] = v
+        elif kind == "pitch":
+            b[c, 1] = v
+        elif kind == "encoder":
+            b[c, 5:] = v
+        elif kind == "noise":
+            m[c] = v
+        else:
+            raise ValueError(f"unknown sensor error kind {kind!r}; expected one of {', '.join(SENSOR_KINDS)}")
+    idx = np.arange(n) % len(cells)
+    return idx, m[idx], b[idx]
+
+
 @torch.no_grad()
 def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None, footsteps=None, delay=None, payload=None,
-            motor=None):
+            motor=None, sensor=None):
     """Reset `env` once and run `steps` control steps of the deterministic `policy` with autoreset off; returns the
     [N, WORDS] float64 device accumulators.  graph=False runs every step eagerly (the same launches, in the same order).
     push = (K, d): after control step K (1 <= K < steps) every env whose episode has not ended gets the heading-frame velocity
@@ -113,13 +142,16 @@ def rollout(env, policy, steps: int, graph: bool = True, push=None, command=None
     footsteps = (mode [N], value [N]): the reset is BatchedHumanoidEnv.reset_footsteps with these plans instead of reset().
     delay = seconds [N]: action delays (BatchedHumanoidEnv.set_action_delay) set after the reset.
     payload = (mass [N], offset (x, y, z)): payloads (BatchedHumanoidEnv.set_payload) set after the reset.
-    motor = strengths [N, act_dim]: motor strengths (BatchedHumanoidEnv.set_motor_strength) set after the reset."""
+    motor = strengths [N, act_dim]: motor strengths (BatchedHumanoidEnv.set_motor_strength) set after the reset.
+    sensor = (noise [N], bias [N, 5 + act_dim]): sensor errors (BatchedHumanoidEnv.set_sensor_errors) set before the reset."""
     if env.eval_words() != WORDS:
         raise RuntimeError(f"the library's evaluation record has {env.eval_words()} words, this module knows {WORDS}")
     if command is not None and env.command_words() != C_WORDS:
         raise RuntimeError(f"the library's command record has {env.command_words()} words, this module knows {C_WORDS}")
     acc = torch.zeros(env.num_envs, WORDS, dtype=torch.float64, device=env.device)
     cacc = torch.zeros(env.num_envs, C_WORDS, dtype=torch.float64, device=env.device) if command is not None else None
+    if sensor is not None:
+        env.set_sensor_errors(*sensor)
     if footsteps is not None:
         env.reset_footsteps(*footsteps)
     else:
@@ -385,6 +417,20 @@ def format_motor_table(d: dict) -> str:
     return _format_cells(d, f"motor strengths on {', '.join(d['joints'])}", "  factor", lambda x: f"{x['factor']:8.3f}")
 
 
+def sensor_summary(acc: np.ndarray, cell: np.ndarray, cells, env_name: str, reward_names) -> dict:
+    """The sensor sweep's outcome per cell: its kind and value, n, and summarize()'s fall fraction, episode length, return,
+    per-mode tracking errors (walking tasks) and footsteps reached and completed (jvrc_step) over the envs of the cell's index."""
+    out = _cell_summary(acc, cell, range(len(cells)), "cell", env_name, reward_names)
+    for x, (kind, v) in zip(out, cells):
+        x["cell"] = int(x["cell"])
+        x.update(kind=kind, value=float(v))
+    return dict(cells=out)
+
+
+def format_sensor_table(d: dict) -> str:
+    return _format_cells(d, "sensor errors", "   kind   value", lambda x: f"{x['kind']:>7s} {x['value']:7.3f}")
+
+
 def format_table(s: dict, max_traj_len: int) -> str:
     L = s["length"]
     lines = [f"{s['num_envs']} environments, one episode each, horizon {max_traj_len} control steps",
@@ -406,7 +452,7 @@ def format_table(s: dict, max_traj_len: int) -> str:
 
 
 def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, push: dict | None = None, commands=None,
-                     footsteps=None, delays=None, payloads=None, motor=None) -> dict:
+                     footsteps=None, delays=None, payloads=None, motor=None, sensor=None) -> dict:
     """Roll `policy` out on every environment of `env` for env.max_traj_len control steps, print the table and, with
     out_report, write the JSON report (meta + summary + per-env arrays).  push = dict(speeds, directions, push_at): the
     push-recovery sweep, with its table and `summary.push`.  commands = [(mode name, value), ...]: the command-tracking sweep
@@ -416,9 +462,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
     with its table and `summary.delay`.  payloads = dict(masses=[kg, ...], at=(x, y, z)): the payload sweep (env i carries the
     mass of cell i mod len(masses) at `at`), with its table and `summary.payload`.  motor = dict(factors=[...], joints=[names],
     mask=[bool per joint]): the motor-strength sweep (env i's masked joints get the factor of cell i mod len(factors), the others 1),
-    with its table and `summary.motor_strength`.  Returns the report."""
-    if sum(x is not None for x in (push, commands, footsteps, delays, payloads, motor)) > 1:
-        raise ValueError("the push, command, footstep, latency, payload and motor-strength sweeps are separate evaluations")
+    with its table and `summary.motor_strength`.  sensor = [(kind, value), ...]: the sensor sweep (env i observes with the
+    errors of cell i mod len(sensor), sensor_grid), with its table and `summary.sensor`.  Returns the report."""
+    if sum(x is not None for x in (push, commands, footsteps, delays, payloads, motor, sensor)) > 1:
+        raise ValueError("the push, command, footstep, latency, payload, motor-strength and sensor sweeps are separate evaluations")
     sweep = held = plans = delay = load = None
     if push is not None:
         k = int(round(push["push_at"] / env.dt))
@@ -438,8 +485,12 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
     if motor is not None:
         factor = motor_grid(env.num_envs, motor["factors"])
         strength = np.where(np.asarray(motor["mask"], dtype=bool)[None, :], factor[:, None], 1.0)
+    rows = cell = None
+    if sensor is not None:
+        cell, noise, bias = sensor_grid(env.num_envs, sensor, env.act_dim)
+        rows = (noise, bias)
     out = rollout(env, policy, env.max_traj_len, push=sweep, command=held, footsteps=plans, delay=delay,
-                  payload=None if load is None else (load, payloads["at"]), motor=strength)
+                  payload=None if load is None else (load, payloads["at"]), motor=strength, sensor=rows)
     acc, cacc = (out[0].cpu().numpy(), out[1].cpu().numpy()) if commands is not None else (out.cpu().numpy(), None)
     summary = summarize(acc, env.model_name, env.reward_names)
     pe = per_env(acc, env.model_name, env.reward_names)
@@ -470,6 +521,10 @@ def evaluate_batched(policy, env, out_report=None, meta: dict | None = None, pus
         summary["motor_strength"] = motor_summary(acc, factor, motor["factors"], motor["joints"], env.model_name, env.reward_names)
         pe.update(motor_strength=factor.tolist())
         print(format_motor_table(summary["motor_strength"]))
+    if sensor is not None:
+        summary["sensor"] = sensor_summary(acc, cell, sensor, env.model_name, env.reward_names)
+        pe.update(sensor_cell=cell.tolist())
+        print(format_sensor_table(summary["sensor"]))
     report = dict(meta or {}, env=env.model_name, precision=env.precision, seed=env.seed, num_envs=env.num_envs,
                   max_traj_len=env.max_traj_len, summary=summary, per_env=pe)
     if out_report is not None:

@@ -33,7 +33,8 @@ from .workers import DeviceRolloutWorker
 # per-env tensors an env may own beside its records (None when off), which a snapshot shard then holds too: the name, what it is
 # and the training flag that turns it on
 _PER_ENV = {"stair_level": ("stair levels", "--stair-curriculum"), "action_delay": ("action delays", "--action-delay"),
-            "payload": ("payloads", "--payload-mass"), "motor_strength": ("motor strengths", "--motor-strength")}
+            "payload": ("payloads", "--payload-mass"), "motor_strength": ("motor strengths", "--motor-strength"),
+            "sensor": ("sensor errors", "--sensor-noise / --sensor-bias")}
 
 
 class _FusedPPOLoss(torch.autograd.Function):

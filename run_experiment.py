@@ -86,6 +86,11 @@ TRAIN_FLAGS = [
                                                          "mass is drawn from U(-R, R)^3 m in the link's frame, R <= 0.25")),
     ("--motor-strength", dict(type=_F, default=0.0, help="random motor strengths: every reset draws each actuated joint's torque scale "
                                                          "from U(1 - R, 1 + R), R in [0, 1] (0: off; DESIGN §7.11)")),
+    ("--sensor-noise", dict(type=_F, default=0.0, help="sensor errors: every env observes its robot state with uniform noise of M times "
+                                                       "the H1 noise scales, M in [0, 4] (0: off; DESIGN §7.12)")),
+    ("--sensor-bias", dict(type=_S, default=None, help="sensor errors: every reset draws its env's IMU roll / pitch offsets from U(-O, O) "
+                                                       "rad, gyro offsets from U(-G, G) rad/s and encoder offsets from U(-E, E) rad, "
+                                                       "given as O,G,E with O, E <= 0.2 and G <= 0.5 (default: none)")),
 ]
 RESUME_FLAGS = [("--path", dict(type=_P, required=True, help="run directory of a `train --snapshot` run")),
                 ("--n-itr", dict(type=_I, default=None, help="PPO iterations in all (default: the run's --n-itr)"))]
@@ -127,7 +132,13 @@ EVAL_FLAGS = [("--path", dict(type=_P, default=None)), ("--logdir", dict(type=_P
                                               "one cell per factor, else exactly one")),
               ("--motor-joints", dict(type=_S, default=None,
                                       help="with --motor-strengths: comma-separated joint names (get_motor_names()) that get the factor, "
-                                           "e.g. R_KNEE,L_KNEE; the others keep 1 (default: every joint)"))]
+                                           "e.g. R_KNEE,L_KNEE; the others keep 1 (default: every joint)")),
+              # the sensor sweep (DESIGN §7.12)
+              ("--sensor-errors", dict(type=_S, nargs="+", action="extend", default=None,
+                                       help="sensor errors KIND:v1,v2,...: roll:RAD and pitch:RAD (IMU offsets, |v| <= 0.2), "
+                                            "encoder:RAD (every motor-position offset, |v| <= 0.2), noise:M (the noise multiplier in "
+                                            "[0, 4]); each value is one cell, the rest of the cell 0; with --num-envs one cell per "
+                                            "value, else exactly one"))]
 ENVS = ("jvrc_walk", "jvrc_step", "h1", "jvrc_walk_terrain", "h1_walk")   # jvrc_walk_terrain is an extension (BASELINE configs[4])
 from learninghumanoidwalking_b200.rl.imitation import TEACHER_FILE  # noqa: E402  the copy of `--imitate` that `resume` uses
 
@@ -162,7 +173,17 @@ def print_system_info(args, training=True):
         motor = getattr(args, "motor_strength", 0.0)
         if motor:
             print(f"Motor strengths: U({1 - motor:g}, {1 + motor:g}) per joint, drawn at every reset")
+        noise, bias = getattr(args, "sensor_noise", 0.0), _sensor_bias(args)
+        if noise or any(bias):
+            print(f"Sensor errors: noise x{noise:g}; offsets up to {bias[0]:g} rad roll / pitch, {bias[1]:g} rad/s gyro, {bias[2]:g} rad "
+                  "encoders, drawn at every reset")
     print("=" * 60)
+
+
+def _sensor_bias(args):
+    """The run's --sensor-bias as (O, G, E): check_sensor_flags leaves it a tuple; a run without the flag has none."""
+    bias = getattr(args, "sensor_bias", None)
+    return (0.0, 0.0, 0.0) if bias is None else tuple(bias)
 
 
 def get_latest_run_dir(logdir):
@@ -214,7 +235,8 @@ def make_env_fn(args, rank, world, local):
                      action_delay=getattr(args, "action_delay", 0.0),   # nor action delays
                      payload_mass=getattr(args, "payload_mass", 0.0),   # nor payloads
                      payload_offset=getattr(args, "payload_offset", 0.0),
-                     motor_strength=getattr(args, "motor_strength", 0.0))   # nor motor strengths
+                     motor_strength=getattr(args, "motor_strength", 0.0),   # nor motor strengths
+                     sensor_noise=getattr(args, "sensor_noise", 0.0), sensor_bias=_sensor_bias(args))   # nor sensor errors
     _env = env_fn()
     if not args.no_mirror:
         try:
@@ -302,6 +324,23 @@ def check_motor_strength_flag(args):
         raise SystemExit(f"train --motor-strength {r}: {e}")
 
 
+def check_sensor_flags(args):
+    """Refuse random sensor errors the env would refuse, before any environment or run directory exists; --sensor-bias O,G,E
+    becomes the tuple (O, G, E) that experiment.pkl keeps."""
+    from learninghumanoidwalking_b200.envs.batched_env import check_sensor_range
+    noise, bias = getattr(args, "sensor_noise", 0.0), getattr(args, "sensor_bias", None)
+    if isinstance(bias, str):
+        try:
+            bias = tuple(float(v) for v in bias.split(","))
+        except ValueError:
+            raise SystemExit(f"train --sensor-bias {bias!r}: expected O,G,E, three comma-separated numbers, e.g. 0.05,0.1,0.02")
+    try:
+        _, bias = check_sensor_range(noise, (0.0, 0.0, 0.0) if bias is None else bias)
+    except ValueError as e:
+        raise SystemExit(f"train --sensor-noise {noise} --sensor-bias {getattr(args, 'sensor_bias', None)}: {e}")
+    args.sensor_bias = bias
+
+
 def _run_cfg(env_name, yaml):
     """The model's cfg block after the user's YAML, as the env applies it."""
     return _run_model(env_name, yaml)["cfg"]
@@ -325,6 +364,7 @@ def run_experiment(args):
     check_action_delay(args)
     check_payload_mass(args)
     check_motor_strength_flag(args)
+    check_sensor_flags(args)
     rank, world, local = _dist_setup()
     timestamp = datetime.now().strftime("%y-%m-%d-%H-%M-%S-%f")[:-3]
     args.logdir = Path(args.logdir) / f"{timestamp}_{args.env}"
@@ -671,6 +711,42 @@ def motor_joint_mask(motor, run_args, yaml):
     return motor["mask"]
 
 
+def sensor_cells(args):
+    """The cells of `eval --sensor-errors KIND:v1,v2 ...` as [(kind, value), ...] (rl/evaluation.py SENSOR_KINDS), or None without
+    the flag; the grammar, the ranges, the cell count and the combinations are refused here, before anything is loaded."""
+    if args.sensor_errors is None:
+        return None
+    from learninghumanoidwalking_b200.envs.batched_env import SENSOR_MAX_BIAS, SENSOR_MAX_NOISE
+    from learninghumanoidwalking_b200.rl.evaluation import SENSOR_KINDS
+    cells = []
+    for spec in args.sensor_errors:
+        kind, _, values = spec.partition(":")
+        if kind not in SENSOR_KINDS:
+            raise SystemExit(f"eval --sensor-errors {spec!r}: unknown kind {kind!r}; expected roll:V[,V...], pitch:V[,V...], "
+                             "encoder:V[,V...] or noise:M[,M...]")
+        try:
+            vs = [float(v) for v in values.split(",")]
+        except ValueError:
+            raise SystemExit(f"eval --sensor-errors {spec!r}: expected {kind}:V[,V...] with comma-separated numbers")
+        lo, hi = (0.0, SENSOR_MAX_NOISE) if kind == "noise" else (-SENSOR_MAX_BIAS[0 if kind != "encoder" else 2],
+                                                                  SENSOR_MAX_BIAS[0 if kind != "encoder" else 2])
+        for v in vs:
+            if not lo <= v <= hi:
+                raise SystemExit(f"eval --sensor-errors {spec!r}: a {kind} value must lie in [{lo:g}, {hi:g}], got {v}")
+        cells += [(kind, v) for v in vs]
+    if (args.push_speeds is not None or args.command is not None or args.footsteps is not None or args.action_delays is not None
+            or args.payloads is not None or args.motor_strengths is not None):
+        raise SystemExit("eval --sensor-errors, --push-speeds, --command, --footsteps, --action-delays, --payloads and "
+                         "--motor-strengths are separate sweeps: run them one at a time")
+    if args.num_envs is None and len(cells) != 1:
+        raise SystemExit(f"eval --sensor-errors: {len(cells)} cells need the batched evaluation (add --num-envs N); the single-env "
+                         "roll-out takes exactly one")
+    if args.num_envs is not None and args.num_envs < len(cells):
+        raise SystemExit(f"eval --num-envs {args.num_envs}: --sensor-errors lists {len(cells)} cells, and every cell needs at least "
+                         "one environment")
+    return cells
+
+
 def check_footstep_env(env_name):
     """Refuse --footsteps for a run whose env is not jvrc_step, before its actor is loaded."""
     if env_name != "jvrc_step":
@@ -690,6 +766,7 @@ def evaluate_batched(args):
     delays = delay_cells(args)
     payloads = payload_cells(args)
     motor = motor_cells(args)
+    sensor = sensor_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -726,7 +803,7 @@ def evaluate_batched(args):
     env = import_env(run_args.env)(args.num_envs, precision=precision, seed=args.seed or 0,
                                    max_traj_len=run_args.max_traj_len, path_to_yaml=yaml)
     report = run(policy, env, args.report, meta=dict(actor=str(path_to_actor), yaml=yaml), push=push, commands=commands,
-                 footsteps=footsteps, delays=delays, payloads=payloads, motor=motor)
+                 footsteps=footsteps, delays=delays, payloads=payloads, motor=motor, sensor=sensor)
     env.close()
     return report
 
@@ -744,6 +821,7 @@ def evaluate(args):
     delays = delay_cells(args)
     payloads = payload_cells(args)
     motor = motor_cells(args)
+    sensor = sensor_cells(args)
     path_to_actor = find_actor(args)
     print(f"Loading model: {path_to_actor}")
     with open(Path(path_to_actor.parent, "experiment.pkl"), "rb") as f:
@@ -770,6 +848,9 @@ def evaluate(args):
     policy = torch.load(path_to_actor, weights_only=False).cuda().eval()
     print_system_info(args, training=False)
     env = import_env(run_args.env)(1, precision=64, seed=args.seed or 0)
+    if sensor is not None:           # the one cell, set once: explicit errors hold through every reset, the first one included
+        from learninghumanoidwalking_b200.rl.evaluation import sensor_grid
+        env.set_sensor_errors(*sensor_grid(1, sensor, env.act_dim)[1:])
 
     def reset():
         if footsteps is not None:     # the one plan, chosen again at every reset
